@@ -1,11 +1,12 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the plugin hook-chain hot path on B200.
+"""bench.py — headline benchmark of the plugin hook-chain hot path on an H100.
 
 Metric (BASELINE.json): tool-call payloads/sec on 16 KiB JSON tool results.
 
   python bench.py --gpus N --steps K --warmup W              # our arm (one process per GPU under torchrun)
   python bench.py --impl reference ...                       # the reference chain's CPU path on the host cores
   python bench.py --workload scan ...                        # BASELINE configs[1] alone: the fused pattern scan (round-1 headline)
+  python bench.py ... --dump-outputs DIR                     # also write what the last timed step computed, DIR/<name>.npy
 
 Default workload = the FULL CHAIN (BASELINE configs[3] semantics at 16 KiB): for every tool result the tool_post_invoke chain
 harmful_content_detector (9 IGNORECASE regexes over every string) -> regex_filter (2 rules, rewrite on match) -> toon_encoder
@@ -31,7 +32,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 PAYLOAD_BYTES = 16384
-UNITS_CHAIN = 32768            # 32768 x 16 KiB = 512 MiB per step per GPU (4x the 126 MB L2)
+UNITS_CHAIN = 32768            # 32768 x 16 KiB = 512 MiB per step per GPU (10x the 50 MB L2)
 UNITS_SCAN = 65536             # scan-only workload: 1 GiB per step per GPU
 DISTINCT = 256                 # distinct seeded payloads, tiled to the batch
 MIX = (("A", 0.5), ("B", 0.25), ("C", 0.25))
@@ -216,7 +217,34 @@ def read_peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet, 3.35 TB/s (not measured)"
+
+
+DUMP_UNITS = 65536            # --dump-outputs: per-unit records of at most this many units (a fixed, seeded sample beyond it)
+TEXT_SAMPLE = 256             # ... and the produced texts of this many of them, one float32 per byte (<= 16 MiB at 16 KiB per text)
+
+
+def dump_sample(n: int, k: int = DUMP_UNITS, seed: int = 0):
+    """Sorted indices of a fixed, seeded sample of k of n items (all of them when n <= k)."""
+    import numpy as np
+
+    return np.arange(n) if n <= k else np.sort(np.random.default_rng(seed).choice(n, k, replace=False))
+
+
+def bitmap_halves(bm):
+    """uint64 match bitmaps as two exact float64 arrays of 32 bits each."""
+    import numpy as np
+
+    bm = np.asarray(bm, dtype=np.uint64)
+    return {"match_bitmap_lo": (bm & np.uint64(0xFFFFFFFF)).astype(np.float64), "match_bitmap_hi": (bm >> np.uint64(32)).astype(np.float64)}
+
+
+def write_outputs(d: str, arrays: dict) -> None:
+    import numpy as np
+
+    os.makedirs(d, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(d, f"{name}.npy"), a)
 
 
 def chain_config(world: int, units: int):
@@ -224,7 +252,7 @@ def chain_config(world: int, units: int):
                         f"on match) + toon_encoder (JSON->TOON, kept when smaller); valid JSON payloads, {int(MIX[0][1]*100)}% tabular / {int(MIX[1][1]*100)}% nested config / "
                         f"{int(MIX[2][1]*100)}% prose-in-JSON, hit rate 1e-4 per word",
             "payload_bytes": PAYLOAD_BYTES, "units_per_gpu": units, "patterns": 11, "pattern_set": "reference defaults (plugins/config.yaml)",
-            "l2_policy": "inputs_larger_than_l2 (512 MiB batch per GPU vs 126 MB L2)",
+            "l2_policy": "inputs_larger_than_l2 (512 MiB batch per GPU vs 50 MB L2)",
             "parallelism": (f"shard{world}: independent payload shards per GPU, one NCCL all_gather of 24-byte verdict records" if world > 1 else "single GPU")}
 
 
@@ -232,7 +260,7 @@ def scan_config(world: int, units: int):
     return {"workload": f"configs[1]: batched 16 KiB payloads ({int(MIX[0][1]*100)}% tabular JSON / {int(MIX[1][1]*100)}% nested JSON / {int(MIX[2][1]*100)}% prose, hit rate 1e-4), "
                         "fused harmful(9 IGNORECASE regex)+deny(3 literals)+regex_filter(2 rules) scan",
             "payload_bytes": PAYLOAD_BYTES, "units_per_gpu": units, "patterns": 14, "pattern_set": "reference defaults (plugins/config.yaml)",
-            "l2_policy": "inputs_larger_than_l2 (1 GiB batch per GPU vs 126 MB L2)",
+            "l2_policy": "inputs_larger_than_l2 (1 GiB batch per GPU vs 50 MB L2)",
             "parallelism": f"shard{world}: independent payload shards per GPU, one NCCL all_gather of verdict bitmaps" if world > 1 else "single GPU"}
 
 
@@ -339,7 +367,10 @@ def main():
     ap.add_argument("--units", type=int, default=0)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--hit-rate", type=float, default=1e-4)
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed as DIR/<name>.npy (float64 / float32, seeded sample)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 3)
     chain = args.workload == "chain"
     if not args.units:
@@ -373,7 +404,7 @@ def main():
     from mcp_context_forge_b200.plugins.harmful_content_detector import DEFAULT_LEXICONS   # product's copy of the reference defaults
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device — the B200 path has no CPU fallback")
+        raise SystemExit("bench.py: no CUDA device — the GPU path has no CPU fallback")
     torch.cuda.set_device(local_rank)
     dist = None
     if world > 1:
@@ -475,10 +506,20 @@ def main():
     toon_ms = [each[i] for i in range(1, kn.value, 2)]
     v_res = last["v"].copy()
     out_res, oo_res = engine.device_output(ctx), last["oo"].copy()       # un-timed copy of the resident outputs, for the parity checks below
+    if args.dump_outputs and rank == 0:
+        idx = dump_sample(n)
+        texts = dump_sample(len(idx), TEXT_SAMPLE, seed=1)
+        starts, ends = oo_res[idx[texts]].astype(np.int64), oo_res[idx[texts] + 1].astype(np.int64)
+        sizes = ends - starts
+        write_outputs(args.dump_outputs, {"unit_index": idx.astype(np.float64), **bitmap_halves(v_res["match_bitmap"][idx]),
+                                          "flags": v_res["flags"][idx].astype(np.float64), "out_len": v_res["out_len"][idx].astype(np.float64),
+                                          "aux": v_res["aux"][idx].astype(np.float64), "text_unit_index": idx[texts].astype(np.float64),
+                                          "text_offsets": np.concatenate([[0], np.cumsum(sizes)]).astype(np.float64),
+                                          "text_bytes": np.concatenate([out_res[a:b] for a, b in zip(starts, ends)] + [np.zeros(0, np.uint8)]).astype(np.float32)})
 
     for _ in range(2):
         step_cabi()
-    cabi_steps = max(3, min(args.steps, 5))
+    cabi_steps = args.steps
     ms_cabi = timed(step_cabi, cabi_steps)
     same = bool((last["v"] == v_res).all()) and bool((last["oo"] == oo_res).all()) and \
         bool((last["out"][: int(oo_res[-1])] == out_res[: int(oo_res[-1])]).all())     # resident outputs == host-buffer outputs, byte for byte
@@ -601,15 +642,7 @@ def main():
     scan_k = sum(scan_ms) / max(1, len(scan_ms))
     alg = nbytes + n_out + 24 * n                      # SURVEY §8(d): N_in + N_out + V (24-byte verdict record per payload)
     achieved = alg / (toon_k / 1e3) / 1e9 if toon_k > 0 else None
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "r02_toon_tp_traffic.json")
-    if os.path.exists(tp):
-        try:
-            with open(tp) as f:
-                tj = json.load(f)
-            traffic = tj.get("dram_bytes_per_launch_scaled_to", {}).get(str(nbytes)) or (tj.get("dram_bytes_per_input_byte", 0) * nbytes or None)
-        except Exception:
-            pass
+    traffic = None          # DRAM bytes per launch: needs a hardware-counter profile, which this benchmark does not take
     line = {
         "metric": METRIC_CHAIN, "value": value, "unit": "payloads/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": ms_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8",
@@ -661,7 +694,7 @@ def scan_bench(args, rank, local_rank, world):
     from mcp_context_forge_b200.plugins.harmful_content_detector import DEFAULT_LEXICONS
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device — the B200 path has no CPU fallback")
+        raise SystemExit("bench.py: no CUDA device — the GPU path has no CPU fallback")
     torch.cuda.set_device(local_rank)
     dist = None
     if world > 1:
@@ -765,9 +798,14 @@ def scan_bench(args, rank, local_rank, world):
     launches = ctx.kernel_launches - l0
     clocks = sampler.stop() if sampler else None
     cand, steps_dfa = ctx.scan_counters()
+    if args.dump_outputs and rank == 0:
+        idx = dump_sample(n)
+        bm = d_bms[0].cpu().numpy().view(np.uint64).reshape(n, W)[idx]
+        write_outputs(args.dump_outputs, {"unit_index": idx.astype(np.float64), **{k + (f"_w{w}" if W > 1 else ""): v
+                                          for w in range(W) for k, v in bitmap_halves(bm[:, w]).items()}})
     for _ in range(2):
         step_e2e()
-    e2e_steps = max(3, min(args.steps, 10))
+    e2e_steps = args.steps
     ms_e2e = timed(step_e2e, e2e_steps, use_events=False)
     torch.cuda.synchronize()
     same = bool((h_bm.cuda() == d_bms[0]).all().item())
@@ -789,16 +827,7 @@ def scan_bench(args, rank, local_rank, world):
     k_ms = kms.value / max(1, kn.value)
     alg_bytes = nbytes + 8 * W * n
     achieved = alg_bytes / (k_ms / 1e3) / 1e9 if k_ms > 0 else None
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "scan_kernel_traffic.json")
-    if os.path.exists(tp):
-        try:
-            with open(tp) as f:
-                tj = json.load(f)
-            if tj.get("stream_bytes") == nbytes:
-                traffic = tj.get("dram_bytes_per_launch")
-        except Exception:
-            pass
+    traffic = None          # DRAM bytes per launch: needs a hardware-counter profile, which this benchmark does not take
     line = {"metric": METRIC_SCAN, "value": value, "unit": "payloads/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_step,
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8",
             "data": f"synthetic: {DISTINCT} distinct seeded payloads tiled to {n} units per GPU", "config": config,

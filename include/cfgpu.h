@@ -1,4 +1,4 @@
-/* cfgpu.h — C ABI of libcfgpu.so, the B200 (sm_100a) implementation of ContextForge's plugin
+/* cfgpu.h — C ABI of libcfgpu.so, the H100 (sm_90a) implementation of ContextForge's plugin
  * hook-chain hot path.  Plain pointers and sizes only; no C++/torch types cross this boundary.
  *
  * What each entry point replaces in the reference (/root/reference):
@@ -29,7 +29,7 @@
  *   cf_run_batch / cf_chain
  *       -> the whole per-request plugin chain over one uploaded batch (mcpgateway/services/tool_service.py:5866-5872)
  *
- * Environment (read once per process; defaults are the measured best on B200):
+ * Environment (read once per process):
  *   CF_SCAN_RESERVE_SMS=k   the persistent scan grid leaves k SMs free (a collective running beside it needs somewhere to go)
  *   CF_SCAN_WARPS / CF_SCAN_LB / CF_SCAN_ACC / CF_SCAN_STAGES   scan kernel variant (16 / 64 / 1 / 3)
  *   CF_PAIR_FILTER=0|1   force the byte / pair prefilter instead of choosing per rule set (tests, measurements)

@@ -1,4 +1,4 @@
-"""mcp_context_forge_b200 — B200-native (sm_100a) implementation of ContextForge's plugin hook-chain
+"""mcp_context_forge_b200 — H100-native (sm_90a) implementation of ContextForge's plugin hook-chain
 hot path: regex_filter / deny_filter / harmful_content_detector scans, the request_logging_masking
 redactor and the toon_encoder, behind the reference's Plugin / PluginManager API.
 

@@ -1,5 +1,5 @@
 """ctypes binding of libcfgpu.so (include/cfgpu.h).  There is no CPU fallback: if the library is
-missing or no B200 is visible, everything here raises."""
+missing or no H100 is visible, everything here raises."""
 from __future__ import annotations
 
 import ctypes
@@ -85,7 +85,7 @@ def load() -> ctypes.CDLL:
     if _lib is not None:
         return _lib
     if not os.path.exists(SO_PATH):
-        raise ImportError(f"{SO_PATH} is missing — run `python -m mcp_context_forge_b200.build` (nvcc, sm_100a). There is no CPU fallback.")
+        raise ImportError(f"{SO_PATH} is missing — run `python -m mcp_context_forge_b200.build` (nvcc, sm_90a). There is no CPU fallback.")
     lib = ctypes.CDLL(SO_PATH)
     for name, (res, args) in _SIGS.items():
         fn = getattr(lib, name)  # AttributeError if the symbol is not exported

@@ -1,4 +1,4 @@
-"""In-tree build of libcfgpu.so (nvcc, sm_100a only).  Used by __graft_entry__.build() and runnable
+"""In-tree build of libcfgpu.so (nvcc, sm_90a only).  Used by __graft_entry__.build() and runnable
 directly: `python -m mcp_context_forge_b200.build [--force] [-v]`.  nvcc cross-compiles without a GPU.
 
 Every source becomes an object under csrc/_obj/ (git-ignored); objects are rebuilt only when the source or a
@@ -18,7 +18,8 @@ OBJ = os.path.join(CSRC, "_obj")
 SO = os.path.join(HERE, "libcfgpu.so")
 INC = os.path.join(os.path.dirname(HERE), "include")
 SOURCES = ["cfgpu.cu", "cfjson.cu", "cfjson_seq.cu", "cf_host.cpp", "re_backend.cpp"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
 
 
 def _nvcc() -> str:
@@ -86,7 +87,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             if verbose:
                 sys.stderr.write(log)
     objs = [os.path.join(OBJ, os.path.splitext(s)[0] + ".o") for s in SOURCES]
-    cmd = [_nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-cudart", "static", "-o", SO] + objs
+    cmd = [_nvcc()] + ARCH + ["-shared", "-cudart", "static", "-o", SO] + objs
     proc = subprocess.run(cmd, capture_output=True, text=True)
     if proc.returncode != 0:
         raise RuntimeError("link failed:\n" + proc.stdout + proc.stderr)

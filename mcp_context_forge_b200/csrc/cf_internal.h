@@ -43,7 +43,7 @@ struct cf_ctx {
   uint32_t prof_used = 0;
   bool prof_on = false;
   // scan kernel configuration (CF_SCAN_WARPS / CF_SCAN_ACC override the defaults; experiments)
-  uint32_t scan_warps = 16;        // best of the measured variants (profiles/README.md)
+  uint32_t scan_warps = 16;        // defaults: see the CF_SCAN_* variables in include/cfgpu.h
   uint32_t scan_lane_bytes = 64;
   uint32_t scan_acc = 1;
   uint32_t scan_stages = 3;

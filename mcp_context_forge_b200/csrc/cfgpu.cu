@@ -1,5 +1,5 @@
 // cfgpu.cu — device half of libcfgpu.so (include/cfgpu.h): contexts, table upload, batches and
-// the sm_100a kernels of the plugin hook-chain hot path.
+// the sm_90a kernels of the plugin hook-chain hot path.
 //
 // Kernel inventory
 //   prep_kernel      per scan: bitmap initialisation (always-match bits), tile -> first-unit index
@@ -817,7 +817,7 @@ int cf_init(int device_ordinal, cf_ctx** out) {
   cudaDeviceProp prop;
   CF_CUDA(ctx, cudaGetDeviceProperties(&prop, device_ordinal));
   ctx->sm_count = prop.multiProcessorCount;
-  if (prop.major < 10) { ctx->err = "libcfgpu.so is built for sm_100a (Blackwell) only"; return CF_E_NOGPU; }
+  if (prop.major != 9 || prop.minor != 0) { ctx->err = "libcfgpu.so is built for sm_90a (Hopper, compute capability 9.0) only"; return CF_E_NOGPU; }
   CF_CUDA(ctx, cudaMalloc(&ctx->d_qstate, 4 * sizeof(uint64_t)));
   CF_CUDA(ctx, cudaMemset(ctx->d_qstate, 0, 4 * sizeof(uint64_t)));
   CF_CUDA(ctx, cudaMalloc(&ctx->d_queue, (size_t)ctx->qcap * sizeof(uint64_t)));

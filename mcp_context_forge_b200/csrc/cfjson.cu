@@ -20,8 +20,8 @@
 //   stage 1b  (CF_INDEX_CLASSIFY) lane-parallel over the tokens: strings validated + their predicates/hash,
 //             scalars validated — the same functions the sequential parser uses
 // Measured as a front end of the TOON / masking kernels (index kernel + token-driven DOM build per lane)
-// it LOSES to the sequential per-lane parser on B200 at large batches (15.8 vs 10.1 ms for 32 768 x 16 KiB:
-// stage 1b is issue-bound at ~12 warp-instructions per byte and the tokens triple the memory traffic), so
+// it loses to the sequential per-lane parser at large batches (stage 1b is issue-bound at ~12 warp-instructions
+// per byte and the tokens triple the memory traffic), so
 // those kernels keep json_parse; the index stands alone as a reusable op (string extraction, length
 // guards) and as the first stage of the token-parallel design the next round needs (DESIGN.md §7).
 // ------------------------------------------------------------------------------------------------

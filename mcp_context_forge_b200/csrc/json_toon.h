@@ -330,8 +330,8 @@ CF_HD bool scan_number(const uint8_t* s, uint32_t n, uint32_t* ppos, uint32_t* p
 }
 
 // Parse `s[0..n)` (a whole JSON document, surrounding whitespace allowed) into nodes[0..cap).
-// Token-at-a-time.  (A byte-at-a-time flat state machine was tried to cut warp divergence and measured
-// 2.4x SLOWER on B200 — profiles/README.md — so the straightforward form stays.)
+// Token-at-a-time.  (A byte-at-a-time flat state machine was tried to cut warp divergence and was
+// slower, so the straightforward form stays.)
 // All per-container running state (child count, last child, kind, the key hashes of the open objects)
 // lives in thread-local arrays: a read-after-write through the node array in HBM costs an L2 round
 // trip per token, local memory stays in L1.  Nodes are written once, when complete.

@@ -726,8 +726,8 @@ static double partition_patterns(const std::vector<PatFilter>& pf, size_t nb, st
   return total();
 }
 
-// expected candidates per byte above which the pair filter (slower per byte, far more selective) takes over;
-// calibrated on B200: the byte filter scans at 4.6 TB/s plus ~0.12 ns per candidate, the pair filter at ~2 TB/s
+// expected candidates per byte above which the pair filter (slower per byte, far more selective) takes over:
+// past it the byte filter spends more time verifying candidates than the pair filter loses on its lower scan rate
 static const double PAIR_MODE_COST = 3e-3;
 
 static void assign_buckets(const std::vector<PatFilter>& pf, FilterOut& fo, bool allow_pairs) {

@@ -1,9 +1,10 @@
-"""Container-only: the whole product chain against the whole reference chain.  One YAML, two managers: the sequential `PluginManager` loading
+"""The whole product chain against the whole reference chain.  One YAML, two managers: the sequential `PluginManager` loading
 the REFERENCE'S OWN plugin classes (kind: plugins.regex_filter.search_replace.SearchReplacePlugin, ... imported unmodified from /root/reference)
 and `BatchedPluginManager` loading this repo's drop-ins (kind: mcp_context_forge_b200.plugins....) on the engine's CPU simulator — same priorities,
 modes, conditions and hook policies, random waves of concurrent requests on the three hooks of the path, violations as results and as
 exceptions.  Every request's (continue_processing, modified payload, violation, metadata) or raised error must be equal.
-usage: python tools/fuzz_chain_vs_reference.py [seed] [rounds] [requests per wave]"""
+With --record the reference itself is run and its answers are stored (tools/ref_answers.py); without it they are read back from tests/golden/.
+usage: python tools/fuzz_chain_vs_reference.py [seed] [rounds] [requests per wave] [--record]"""
 import asyncio
 import json
 import os
@@ -17,6 +18,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 import gen_golden  # noqa: E402
+from ref_answers import Answers, canon  # noqa: E402
 
 OURS = {"harm": "mcp_context_forge_b200.plugins.harmful_content_detector.HarmfulContentDetectorPlugin", "deny": "mcp_context_forge_b200.plugins.deny_filter.DenyListPlugin",
         "regex": "mcp_context_forge_b200.plugins.regex_filter.SearchReplacePlugin", "sql": "mcp_context_forge_b200.plugins.sql_sanitizer.SQLSanitizerPlugin",
@@ -68,12 +70,12 @@ def render(plugs, kinds, fail_all=False):
 
 
 def main() -> int:
-    if not os.path.isdir(gen_golden.REF):
-        print("fuzz_chain_vs_reference: /root/reference is not here (container-only tool)")
-        return 0
-    seed = int(sys.argv[1]) if len(sys.argv) > 1 else 1
-    rounds = int(sys.argv[2]) if len(sys.argv) > 2 else 20
-    nreq = int(sys.argv[3]) if len(sys.argv) > 3 else 60
+    record = "--record" in sys.argv
+    argv = [a for a in sys.argv[1:] if a != "--record"]
+    seed = int(argv[0]) if len(argv) > 0 else 1
+    rounds = int(argv[1]) if len(argv) > 1 else 20
+    nreq = int(argv[2]) if len(argv) > 2 else 60
+    answers = Answers("chain", [seed, rounds, nreq], record)
     gen_golden.install_shims()
     import logging
 
@@ -98,9 +100,10 @@ def main() -> int:
             fail_all = rng.random() < 0.2
             open(a, "w").write(render(plugs, REFS, fail_all))
             open(b, "w").write(render(plugs, OURS, fail_all))
-            seq = fw.PluginManager(a, timeout=120, hook_policies=tm.POL)
+            seq = fw.PluginManager(a, timeout=120, hook_policies=tm.POL) if record else None
             bat = BatchedPluginManager(b, timeout=120, hook_policies=tm.POL, max_wave=rng.choice([8192, 8192, 7, 1, 33]), window_us=rng.choice([0, 0, 50, 400]))
-            loop.run_until_complete(seq.initialize())
+            if record:
+                loop.run_until_complete(seq.initialize())
             try:
                 loop.run_until_complete(bat.initialize())
             except (UnsupportedPattern, RuntimeError) as exc:
@@ -132,16 +135,17 @@ def main() -> int:
                 for vae in (False, True):
                     async def wave(m):
                         return await asyncio.gather(*[m.invoke_hook(hook, p, g, None, vae) for p, g in zip(pls, gcs)], return_exceptions=True)
-                    x = loop.run_until_complete(wave(seq))
+                    x = answers(lambda: [tm.norm(u) for u in loop.run_until_complete(wave(seq))])
                     y = loop.run_until_complete(wave(bat))
                     for i, (u, v) in enumerate(zip(x, y)):
                         n += 1
-                        if tm.norm(u) != tm.norm(v):
+                        if u != canon(tm.norm(v)):
                             bad += 1
                             if bad <= 5:
-                                print("BAD", hook, "vae", vae, "\n  chain    ", [(p["k"], p["mode"], p["priority"]) for p in plugs], "\n  payload  ", repr(pls[i])[:400], "\n  reference", repr(tm.norm(u))[:600],
+                                print("BAD", hook, "vae", vae, "\n  chain    ", [(p["k"], p["mode"], p["priority"]) for p in plugs], "\n  payload  ", repr(pls[i])[:400], "\n  reference", repr(u)[:600],
                                       "\n  product  ", repr(tm.norm(v))[:600])
             slow += bat.slow_path_calls
+    answers.finish()
     print(f"seed={seed} chains={rounds} rejected_loudly={rejected} requests={n} slow_path_calls={slow} bad={bad} time={time.time() - t0:.1f}s")
     return 1 if bad else 0
 

@@ -1,7 +1,8 @@
-"""Container-only: live differential fuzz of the json_repair drop-in (on the engine's CPU simulator: JSON kernel source for "does it parse",
+"""Differential fuzz of the json_repair drop-in (on the engine's CPU simulator: JSON kernel source for "does it parse",
 substitution routines for the trailing-comma rule) against the REFERENCE'S OWN plugins/json_repair/json_repair.py, imported unmodified from
 /root/reference (orjson stood in for by the strict stdlib parser; texts that would expose an orjson / json delta are skipped).
-usage: python tools/fuzz_json_repair_vs_reference.py [seed] [cases]"""
+With --record the reference itself is run and its answers are stored (tools/ref_answers.py); without it they are read back from tests/golden/.
+usage: python tools/fuzz_json_repair_vs_reference.py [seed] [cases] [--record]"""
 import os
 import random
 import re
@@ -14,28 +15,37 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 import gen_golden  # noqa: E402
 from fuzz_toon_tp import make_gen  # noqa: E402
+from ref_answers import Answers  # noqa: E402
 
 _DELTA = re.compile(r"\d{18,}|[eE][+-]?\d{3,}|\\u[dD][89a-fA-F]|NaN|Infinity")
 
 
 def main() -> int:
-    if not os.path.isdir(gen_golden.REF):
-        print("fuzz_json_repair_vs_reference: /root/reference is not here (container-only tool)")
-        return 0
-    seed = int(sys.argv[1]) if len(sys.argv) > 1 else 1
-    n = int(sys.argv[2]) if len(sys.argv) > 2 else 3000
+    record = "--record" in sys.argv
+    argv = [a for a in sys.argv[1:] if a != "--record"]
+    seed = int(argv[0]) if len(argv) > 0 else 1
+    n = int(argv[1]) if len(argv) > 1 else 3000
+    answers = Answers("json_repair", [seed, n], record)
     gen_golden.install_shims()
     import pytest
     from cpex.framework import GlobalContext, PluginConfig, PluginContext, ToolPostInvokePayload
-    from plugins.json_repair.json_repair import JSONRepairPlugin as RefPlugin
 
     import hostsim_batcher
     import test_json_repair as tj
     from mcp_context_forge_b200.plugins.json_repair import JSONRepairPlugin
 
     hostsim_batcher.install(pytest.MonkeyPatch())
-    ref = RefPlugin(PluginConfig(name="jr", kind="x", hooks=["tool_post_invoke"]))
+    if record:
+        from plugins.json_repair.json_repair import JSONRepairPlugin as RefPlugin
+
+        ref = RefPlugin(PluginConfig(name="jr", kind="x", hooks=["tool_post_invoke"]))
     ctx = PluginContext(global_context=GlobalContext(request_id="fuzz"))
+
+    def reference(t):
+        r = gen_golden.run(ref.tool_post_invoke(ToolPostInvokePayload(name="t", result=t), ctx))
+        return {"continue_processing": r.continue_processing, "out_result": r.modified_payload.result if r.modified_payload is not None else None,
+                "modified": r.modified_payload is not None, "metadata": r.metadata or {}}
+
     rng = random.Random(seed)
     case = make_gen(rng)
     t0 = time.time()
@@ -52,15 +62,14 @@ def main() -> int:
         t = rng.choice(["", "", " ", "\n", " ", "\t"]) + t + rng.choice(["", "", " ", "\r\n", "　"])
         if _DELTA.search(t) or any(0xD800 <= ord(c) <= 0xDFFF for c in t) or t.count("[") + t.count("{") > 60:
             continue
-        r = gen_golden.run(ref.tool_post_invoke(ToolPostInvokePayload(name="t", result=t), ctx))
-        cases.append({"result": t, "continue_processing": r.continue_processing, "out_result": r.modified_payload.result if r.modified_payload is not None else None,
-                      "modified": r.modified_payload is not None, "metadata": r.metadata or {}})
+        cases.append({"result": t, **answers(lambda: reference(t))})
     try:
         for i in range(0, len(cases), 500):
             tj.check_dropin(cases[i:i + 500], JSONRepairPlugin)
     except AssertionError as exc:
         print("BAD", str(exc)[:1500])
         return 1
+    answers.finish()
     print(f"seed={seed} cases={len(cases)} repaired={sum(c['modified'] for c in cases)} bad=0 time={time.time() - t0:.1f}s")
     return 0
 

@@ -1,8 +1,9 @@
-"""Container-only: live differential fuzz of the masker's source (csrc/json_mask.h on the host build: key classifier, depth rule, key order,
+"""Differential fuzz of the masker's source (csrc/json_mask.h on the host build: key classifier, depth rule, key order,
 serialisation) against the REFERENCE'S OWN Python twin of the Rust crate (`mcpgateway/middleware/request_logging_middleware.py:83-291`, its pure
 functions exec'd unmodified from /root/reference as tools/gen_golden.py does) — generated key names (token vocabulary x separators x casings),
 random nested bodies, max_depth 0..12 — and against the oracle (oracle/mask_ref.py) byte for byte.
-usage: python tools/fuzz_mask_vs_reference.py [seed] [keys] [bodies]"""
+With --record the reference itself is run and its answers are stored (tools/ref_answers.py); without it they are read back from tests/golden/.
+usage: python tools/fuzz_mask_vs_reference.py [seed] [keys] [bodies] [--record]"""
 import json
 import os
 import random
@@ -16,6 +17,7 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 import gen_golden  # noqa: E402
 import hostsim_util as hs  # noqa: E402
 from oracle import mask_ref  # noqa: E402
+from ref_answers import Answers, canon  # noqa: E402
 
 VOCAB = ["auth", "token", "tokens", "tokenizer", "secret", "secrets", "key", "keys", "api", "jwt", "pass", "password", "passwd", "pwd", "word", "phrase", "session", "id", "count",
          "status", "private", "client", "access", "refresh", "cookie", "x", "url", "ttl", "hash", "name", "type", "o", "oauth", "credential", "cred", "bearer", "signature", "sig",
@@ -40,14 +42,15 @@ def make_key(rng):
 
 
 def main() -> int:
-    if not os.path.isdir(gen_golden.REF):
-        print("fuzz_mask_vs_reference: /root/reference is not here (container-only tool)")
-        return 0
-    seed = int(sys.argv[1]) if len(sys.argv) > 1 else 1
-    nkeys = int(sys.argv[2]) if len(sys.argv) > 2 else 20000
-    nbodies = int(sys.argv[3]) if len(sys.argv) > 3 else 2000
-    gen_golden.install_shims()
-    ns = gen_golden.load_masking_twin()
+    record = "--record" in sys.argv
+    argv = [a for a in sys.argv[1:] if a != "--record"]
+    seed = int(argv[0]) if len(argv) > 0 else 1
+    nkeys = int(argv[1]) if len(argv) > 1 else 20000
+    nbodies = int(argv[2]) if len(argv) > 2 else 2000
+    answers = Answers("mask", [seed, nkeys, nbodies], record)
+    if record:
+        gen_golden.install_shims()
+    ns = gen_golden.load_masking_twin() if record else None
     rng = random.Random(seed)
     t0 = time.time()
     bad = 0
@@ -57,7 +60,7 @@ def main() -> int:
         if k in seen:
             continue
         seen.add(k)
-        exp = bool(ns["_is_sensitive_key"](k))
+        exp = answers(lambda: bool(ns["_is_sensitive_key"](k)))
         got = hs.key_sensitive_host(k)
         orc = mask_ref.is_sensitive_key(k)
         if not (exp == got == orc):
@@ -95,12 +98,12 @@ def main() -> int:
     for _ in range(nbodies):
         obj = rand_obj(rng.randint(1, 7))
         md = rng.choice([10, 10, 3, 1, 0, 2, 12, 5])
-        exp = ns["mask_sensitive_data"](obj, md)
+        exp = answers(lambda: ns["mask_sensitive_data"](obj, md))
         body = json.dumps(obj, ensure_ascii=rng.random() < 0.5, separators=rng.choice([(",", ":"), (", ", ": ")])).encode()
         st, out = hs.mask_host(body, md)
         orc = mask_ref.mask_json_bytes(body, md)
         nb += 1
-        if st != 0 or out != orc or json.loads(out) != json.loads(json.dumps(exp)):
+        if st != 0 or out != orc or json.loads(out) != exp:
             bad += 1
             if bad <= 10:
                 print("BODY", body[:300], md, "\n  reference", json.dumps(exp)[:300], "\n  kernel   ", st, (out or b"")[:300], "\n  oracle   ", orc[:300])
@@ -124,19 +127,19 @@ def main() -> int:
     for _ in range(nbodies // 4):
         obj = rand_obj(rng.randint(1, 6))
         md = rng.choice([10, None, 3, 1, 0, 2])
-        exp = ns["mask_sensitive_data"](obj, 10 if md is None else md)
-        got = mod.mask_sensitive_data(obj, md)
+        exp = answers(lambda: ns["mask_sensitive_data"](obj, 10 if md is None else md))
+        got = canon(mod.mask_sensitive_data(obj, md))
         h = {rng.choice(keys + ["Cookie", "cookie", "COOKIE", "CooKie", "Content-Type", "Accept"]): rng.choice(cookies) for _ in range(rng.randint(0, 6))}
-        hexp, hgot = ns["mask_sensitive_headers"](h), mod.mask_sensitive_headers(h)
+        hexp, hgot = answers(lambda: ns["mask_sensitive_headers"](h)), canon(mod.mask_sensitive_headers(h))
         nm += 2
-        if got != exp or hexp != hgot or masking.mask_sensitive_headers_batch([h, h])[1] != hexp:
+        if got != exp or hexp != hgot or canon(masking.mask_sensitive_headers_batch([h, h])[1]) != hexp:
             bad += 1
             if bad <= 10:
                 print("MODULE", repr(obj)[:200], md, "\n  reference", repr(exp)[:200], "\n  module   ", repr(got)[:200], "\n  headers", h, "\n  reference", hexp, "\n  module   ", hgot)
     words = ["password", "PassWord", "pass phrase", "secret", "SECRET", "toKen", "\u212aey", "api_\u212aey", "api-key", "APIKEY", "apikey", "access_token", "refresh-token", "client_secret",
              "Authorization", "auth_token", "jwt_token", "private_key", "private key", "İ", "ſecret", "hello", "x=1", "{", "\xff", "日本", " ", "&", "tok", "en"]
     bodies = [("".join(rng.choice(words) + rng.choice(["", " ", "=", "&", "\n"]) for _ in range(rng.randint(0, 6)))).encode("utf-8", "ignore") + rng.choice([b"", b"\xfe", b"\xc3"]) for _ in range(nbodies // 4)]
-    lows = tuple(ns["SENSITIVE_KEYS"])
+    lows = tuple(answers(lambda: list(ns["SENSITIVE_KEYS"])))
     exp_fb = []
     for b_ in bodies:
         s_ = b_.decode("utf-8", errors="ignore")                      # request_logging_middleware.py:661-667
@@ -148,6 +151,7 @@ def main() -> int:
             bad += 1
             if bad <= 10:
                 print("FALLBACK", b_, "reference", repr(e_), "module", repr(g_))
+    answers.finish()
     print(f"seed={seed} keys={len(seen)} bodies={nb} module_calls={nm} bad={bad} time={time.time() - t0:.1f}s")
     return 1 if bad else 0
 

@@ -1,9 +1,10 @@
-"""Container-only: live differential fuzz of the drop-in PLUGINS (their host logic — unit extraction, verdict -> result assembly, findings
+"""Differential fuzz of the drop-in PLUGINS (their host logic — unit extraction, verdict -> result assembly, findings
 order, payload rebuilding — on the engine's CPU simulator) against the REFERENCE'S OWN plugin classes, imported unmodified from /root/reference:
 regex_filter, deny_filter, harmful_content_detector, sql_sanitizer, code_safety_linter, toon_encoder.  Random configurations (from pools that
 include rules matching "", group-reference templates, invalid patterns, IGNORECASE Unicode traps) and random payload shapes (nested dicts /
 lists / non-strings, every hook each plugin implements).  A configuration the engine rejects loudly (UnsupportedPattern) is skipped and counted.
-usage: python tools/fuzz_plugins_vs_reference.py [seed] [rounds]"""
+With --record the reference itself is run and its answers are stored (tools/ref_answers.py); without it they are read back from tests/golden/.
+usage: python tools/fuzz_plugins_vs_reference.py [seed] [rounds] [--record]"""
 import asyncio
 import json
 import os
@@ -16,6 +17,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 import gen_golden  # noqa: E402
+from ref_answers import Answers  # noqa: E402
 
 WORDS = ["kill", "myself", "suicide", "self-harm", "want", "to", "die", "him", "her", "them", "someone", "shoot", "stab", "eradicate", "people", "racial", "slur", "hate", "speech", "crap",
          "crud", "innovative", "groundbreaking", "revolutionary", "the", "a", "of", "x", "Kill", "KILL", "ſuicide", "Kill", "é", "ß", "naïve", "日本語", "\U0001f600", "12", "_", "-", ".",
@@ -67,20 +69,23 @@ def norm(r):
 
 
 def main() -> int:
-    if not os.path.isdir(gen_golden.REF):
-        print("fuzz_plugins_vs_reference: /root/reference is not here (container-only tool)")
-        return 0
-    seed = int(sys.argv[1]) if len(sys.argv) > 1 else 1
-    rounds = int(sys.argv[2]) if len(sys.argv) > 2 else 40
+    record = "--record" in sys.argv
+    argv = [a for a in sys.argv[1:] if a != "--record"]
+    seed = int(argv[0]) if len(argv) > 0 else 1
+    rounds = int(argv[1]) if len(argv) > 1 else 40
+    answers = Answers("plugins", [seed, rounds], record)
     gen_golden.install_shims()
     import pytest
     from cpex.framework import GlobalContext, PluginConfig, PluginContext, PromptPosthookPayload, PromptPrehookPayload, ToolPostInvokePayload, ToolPreInvokePayload
-    from plugins.code_safety_linter.code_safety_linter import CodeSafetyLinterPlugin as RCode
-    from plugins.deny_filter.deny import DenyListPlugin as RDeny
-    from plugins.harmful_content_detector.harmful_content_detector import HarmfulContentDetectorPlugin as RHarm
-    from plugins.regex_filter.search_replace import SearchReplacePlugin as RRegex
-    from plugins.sql_sanitizer.sql_sanitizer import SQLSanitizerPlugin as RSql
-    from plugins.toon_encoder.toon_encoder import ToonEncoderPlugin as RToon
+    if record:
+        from plugins.code_safety_linter.code_safety_linter import CodeSafetyLinterPlugin as RCode
+        from plugins.deny_filter.deny import DenyListPlugin as RDeny
+        from plugins.harmful_content_detector.harmful_content_detector import HarmfulContentDetectorPlugin as RHarm
+        from plugins.regex_filter.search_replace import SearchReplacePlugin as RRegex
+        from plugins.sql_sanitizer.sql_sanitizer import SQLSanitizerPlugin as RSql
+        from plugins.toon_encoder.toon_encoder import ToonEncoderPlugin as RToon
+    else:
+        RCode = RDeny = RHarm = RRegex = RSql = RToon = None
 
     import hostsim_batcher
     from mcp_context_forge_b200.plugins.code_safety_linter import CodeSafetyLinterPlugin
@@ -120,7 +125,7 @@ def main() -> int:
         ]
         for name, rcls, ocls, cfg, hooks in plan:
             pc = PluginConfig(name=name, kind="x", hooks=hooks, config=cfg)
-            ref = rcls(pc)
+            ref = rcls(pc) if record else None
             try:
                 ours = ocls(pc)
             except UnsupportedPattern:
@@ -141,10 +146,13 @@ def main() -> int:
                         pa, pb = mk(), mk()
                     except Exception:  # noqa: BLE001 - a payload shape the model rejects
                         continue
-                    try:
-                        exp = norm(loop.run_until_complete(getattr(ref, hook)(pa, ctx)))
-                    except Exception as exc:  # noqa: BLE001 - the reference raises: so must the drop-in
-                        exp = {"raises": type(exc).__name__, "message": str(exc)}
+                    def reference():
+                        try:
+                            return norm(loop.run_until_complete(getattr(ref, hook)(pa, ctx)))
+                        except Exception as exc:  # noqa: BLE001 - the reference raises: so must the drop-in
+                            return {"raises": type(exc).__name__, "message": str(exc)}
+
+                    exp = answers(reference)
                     try:
                         got = norm(loop.run_until_complete(getattr(ours, hook)(pb, ctx)))
                     except Exception as exc:  # noqa: BLE001
@@ -156,12 +164,14 @@ def main() -> int:
                         if bad <= 6:
                             print("BAD", name, hook, repr(cfg)[:300], "\n  payload  ", repr(p)[:400], "\n  reference", json.dumps(exp, ensure_ascii=False)[:500],
                                   "\n  drop-in  ", json.dumps(got, ensure_ascii=False)[:500])
-            if callable(getattr(ref, "get_stats", None)) and callable(getattr(ours, "get_stats", None)):      # toon_encoder's counters after the same calls
+            if callable(getattr(ours, "get_stats", None)):      # toon_encoder's counters after the same calls
                 n += 1
-                if ref.get_stats() != ours.get_stats():
+                exp = answers(lambda: ref.get_stats() if callable(getattr(ref, "get_stats", None)) else None)
+                if exp is not None and exp != json.loads(json.dumps(ours.get_stats())):
                     bad += 1
                     if bad <= 6:
-                        print("BAD stats", name, repr(cfg), ref.get_stats(), ours.get_stats())
+                        print("BAD stats", name, repr(cfg), exp, ours.get_stats())
+    answers.finish()
     print(f"seed={seed} rounds={rounds} hook_calls={n} configs_rejected_loudly={rejected} reference_raised={raised} bad={bad} time={time.time() - t0:.1f}s")
     return 1 if bad else 0
 

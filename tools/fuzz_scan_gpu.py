@@ -1,5 +1,5 @@
 """Random-pattern differential test of the GPU scan (both prefilter kernels) against CPython `re`.
-usage: [CF_PAIR_FILTER=0|1] python -u tools/fuzz_scan_gpu.py [first_seed] [rounds]   (needs a B200)"""
+usage: [CF_PAIR_FILTER=0|1] python -u tools/fuzz_scan_gpu.py [first_seed] [rounds]   (needs an H100)"""
 import random
 import re
 import sys

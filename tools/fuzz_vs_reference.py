@@ -1,9 +1,10 @@
-"""Container-only: live differential fuzz of the TOON kernels' source (sequential encoder csrc/json_toon.h on the host build; token-parallel kernel
+"""Differential fuzz of the TOON kernels' source (sequential encoder csrc/json_toon.h on the host build; token-parallel kernel
 body csrc/json_tp.h on the 32-fibre warp emulator) against the REFERENCE'S OWN `plugins/toon_encoder/toon.py`, imported unmodified from
 /root/reference — no restatement in between (the oracle is compared too, so a gap in it shows).  Random JSON documents from the generator of
 tools/fuzz_toon_tp.py (adversarial keys / strings / numbers, tables, byte-level mutations).  orjson is not installable here: the strict stdlib
 parser stands in, and documents that would expose an orjson / json delta (integers beyond 64 bits, lone surrogates, non-finite floats) are skipped.
-usage: python tools/fuzz_vs_reference.py [seed] [cases] [gen1|gen2|synth]"""
+With --record the reference itself is run and its answers are stored (tools/ref_answers.py); without it they are read back from tests/golden/.
+usage: python tools/fuzz_vs_reference.py [seed] [cases] [gen1|gen2|synth] [--record]"""
 import importlib.util
 import json
 import math
@@ -21,6 +22,7 @@ import hostsim_util as hs  # noqa: E402
 from fuzz_toon_tp import make_gen  # noqa: E402
 from mcp_context_forge_b200.plugins.toon_encoder import _encode_error  # noqa: E402
 from oracle import toon_ref  # noqa: E402
+from ref_answers import Answers  # noqa: E402
 
 
 def load_reference_toon():
@@ -46,8 +48,8 @@ def delta_free(v) -> bool:
 
 
 def expected(toon, t: str):
-    """(status, text) as include/cfgpu.h defines them for an unlimited output buffer: 0 = the reference's toon.encode(orjson.loads(t)),
-    2 = not JSON, 3 / 4 = toon.encode raises ValueError / AttributeError."""
+    """(status, text, exception message) as include/cfgpu.h defines them for an unlimited output buffer: 0 = the reference's
+    toon.encode(orjson.loads(t)), 2 = not JSON, 3 / 4 = toon.encode raises ValueError / AttributeError."""
     try:
         t.encode("utf-8")
     except UnicodeEncodeError:
@@ -55,17 +57,15 @@ def expected(toon, t: str):
     try:
         doc = json.loads(t, parse_constant=lambda c: (_ for _ in ()).throw(ValueError(c)))
     except (ValueError, RecursionError):
-        return (2, None)
+        return (2, None, None)
     if not delta_free(doc):
         return None
     try:
-        return (0, toon.encode(doc))
+        return (0, toon.encode(doc), None)
     except ValueError as exc:
-        expected.message = str(exc)
-        return (3, None)
+        return (3, None, str(exc))
     except AttributeError as exc:
-        expected.message = str(exc)
-        return (4, None)
+        return (4, None, str(exc))
 
 
 def make_gen2(rng):
@@ -138,14 +138,14 @@ def make_gen2(rng):
 
 
 def main() -> int:
-    if not os.path.isdir(REF):
-        print("fuzz_vs_reference: /root/reference is not here (container-only tool)")
-        return 0
-    seed = int(sys.argv[1]) if len(sys.argv) > 1 else 1
-    n = int(sys.argv[2]) if len(sys.argv) > 2 else 2000
-    toon = load_reference_toon()
+    record = "--record" in sys.argv
+    argv = [a for a in sys.argv[1:] if a != "--record"]
+    seed = int(argv[0]) if len(argv) > 0 else 1
+    n = int(argv[1]) if len(argv) > 1 else 2000
+    which = argv[2] if len(argv) > 2 else "gen1"
+    answers = Answers("toon", [seed, n, which], record)
+    toon = load_reference_toon() if record else None
     rng = random.Random(seed)
-    which = sys.argv[3] if len(sys.argv) > 3 else "gen1"
     if which == "synth":                                        # the bench's payload shapes (tabular / nested config / prose in JSON), 200 B .. 70 KB
         from mcp_context_forge_b200 import synth
 
@@ -159,10 +159,11 @@ def main() -> int:
     done = skipped = handed = bad = worded = 0
     for it in range(n):
         t = case()
-        exp = expected(toon, t)
-        if exp is None or (exp[0] == 2 and any(0xD800 <= ord(c) <= 0xDFFF for c in t)):
+        r = answers(lambda: expected(toon, t))
+        if r is None or (r[0] == 2 and any(0xD800 <= ord(c) <= 0xDFFF for c in t)):
             skipped += 1
             continue
+        exp, message = (r[0], r[1]), r[2]
         done += 1
         seq = hs.toon_host(t, unlimited=True)
         tp = hs.toon_tp(t, unlimited=True, report_errors=True, order=(it & 1) | (rng.randrange(16) << 4))
@@ -178,10 +179,10 @@ def main() -> int:
         if exp[0] in (3, 4):                                    # the wording the drop-in gives the exception (skip_on_error: false) == the reference's
             worded += 1
             msg = str(_encode_error(exp[0], t))
-            if msg != expected.message:
+            if msg != message:
                 bad += 1
                 if bad <= 8:
-                    print("BAD MESSAGE", repr(t)[:400], "\n   reference", expected.message, "\n   drop-in  ", msg)
+                    print("BAD MESSAGE", repr(t)[:400], "\n   reference", message, "\n   drop-in  ", msg)
         # the product's rule on top (include/cfgpu.h): the text is kept only when strictly smaller than the JSON it came from
         small = exp if (exp[0] != 0 or len(exp[1].encode("utf-8")) < len(t.encode("utf-8"))) else (1, None)
         seq2, tp2 = hs.toon_host(t), hs.toon_tp(t, report_errors=True)
@@ -195,6 +196,7 @@ def main() -> int:
             bad += 1
             if bad <= 8:
                 print("BAD", repr(t)[:400], "\n   reference", repr(exp)[:300], "\n   seq      ", repr(seq)[:300], "\n   tp       ", repr(tp)[:300], "\n   oracle   ", repr(orc)[:300])
+    answers.finish()
     print(f"seed={seed} cases={n} compared={done} skipped={skipped} handed_over={handed} error_messages_compared={worded} bad={bad} time={time.time() - t0:.1f}s")
     return 1 if bad else 0
 
