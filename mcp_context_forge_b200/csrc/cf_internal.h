@@ -93,7 +93,8 @@ struct cf_batch {
   uint32_t cap_units = 0;
   uint64_t nbytes = 0;
   uint32_t n = 0;
-  uint64_t generation = 0;         // bumped by every upload
+  uint64_t generation = 0;         // serial of the current upload, unique in the process (0 = none yet): a batch allocated
+                                   // at a freed batch's address never repeats its (address, generation) cache key
   CUtensorMap tmap;                // 2-D view of d_buf: rows of 128 B, box = one scan tile, SWIZZLE_128B
 };
 

@@ -15,6 +15,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <atomic>
 #include <string>
 #include <vector>
 
@@ -1014,7 +1015,8 @@ int cf_batch_upload(cf_ctx* ctx, cf_batch* b, const uint8_t* stream, uint64_t st
   CF_CUDA(ctx, cudaMemcpyAsync(d_stream, stream, stream_bytes, cudaMemcpyHostToDevice, st));
   b->nbytes = stream_bytes;
   b->n = n_units;
-  b->generation++;
+  static std::atomic<uint64_t> upload_serial{0};
+  b->generation = ++upload_serial;
   return CF_OK;
 }
 

@@ -490,7 +490,8 @@ struct Big {
   CF_HD bool shl(uint32_t bits) {
     uint32_t ws = bits >> 5, bs = bits & 31;
     if (n == 0) return true;
-    if (n + ws + 1 > BIGN) return false;
+    const uint32_t carry_word = bs && (w[n - 1] >> (32 - bs)) ? 1u : 0u;   // the top word spills into a new one
+    if (n + ws + carry_word > BIGN) return false;                          // exact: a result that fits is never refused
     for (uint32_t i = n; i-- > 0;) w[i + ws] = w[i];
     for (uint32_t i = 0; i < ws; ++i) w[i] = 0;
     n += ws;

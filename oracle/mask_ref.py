@@ -219,8 +219,8 @@ def parse_serde(payload: bytes) -> Any:
     def parse_int(t: str):
         v = int(t)
         if t.startswith("-"):
-            return v if v != 0 and v >= -(2 ** 63) else float(t)      # "-0" is the float -0.0 in serde_json
-        return v if v <= 2 ** 64 - 1 else float(t)
+            return v if v != 0 and v >= -(2 ** 63) else parse_float(t)      # "-0" is the float -0.0 in serde_json
+        return v if v <= 2 ** 64 - 1 else parse_float(t)                  # beyond binary64 too: "number out of range"
 
     def parse_float(t: str):
         v = float(t)

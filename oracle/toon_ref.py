@@ -233,9 +233,9 @@ def loads_strict(text: str) -> Any:
     def parse_int(t):
         # orjson (yyjson) returns Python ints only inside [-2**63, 2**64-1]; larger integer literals
         # come back as floats (SURVEY.md Appendix A-7; orjson itself is not installable here, so this
-        # rule is restated, not observed)
+        # rule is restated, not observed); one beyond binary64 is rejected like a float literal that overflows
         v = int(t)
-        return v if -(2 ** 63) <= v <= 2 ** 64 - 1 else float(t)
+        return v if -(2 ** 63) <= v <= 2 ** 64 - 1 else parse_float(t)
 
     def parse_float(t):
         v = float(t)
