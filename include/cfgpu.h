@@ -133,7 +133,10 @@ int cf_scan_host(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint8_t* stream, ui
  * that was last uploaded (Python `pattern.sub(replacement, value)` rule after rule,
  * plugins/regex_filter/search_replace.py:127-130).  Rewritten units are returned back to back in
  * out_bytes with out_offsets[n_sel+1]; a unit no rule matched comes back unchanged.
- * CF_E_CAPACITY with *out_needed set when out_cap is too small.  Synchronous. */
+ * There is no limit on the number of rules (the kernel takes 32 per launch and continues each unit in the next launch).
+ * CF_E_CAPACITY with *out_needed set when out_cap is too small (CF_E_CAPACITY without it: a unit would grow beyond 4 GB).
+ * CF_E_TOO_LARGE when a rule's output outgrows the rules' worst-case growth bound (an internal error; cf_last_error names
+ * the unit and the rule).  Synchronous. */
 int cf_sub_host(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint32_t* units, uint32_t n_sel, uint8_t* out_bytes,
                 uint64_t out_cap, uint64_t* out_offsets, uint64_t* out_needed);
 

@@ -575,11 +575,13 @@ static const ScanVariant* scan_variant(uint32_t warps, uint32_t lane_bytes, uint
 // regex_filter substitution (rare path: only units the scan flagged as containing some rule match).
 // One warp per selected unit; rules are applied one after another on the unit's current text
 // (plugins/regex_filter/search_replace.py:127-130), each rule = Python `pattern.sub(repl, text)`:
-// leftmost-first, non-overlapping matches (patterns that can match "" are rejected at compile time).
+// leftmost-first, non-overlapping matches; a rule that can match "" follows re.sub's empty-match rules.  Every write is clamped
+// to the unit's scratch bound, so a bound that is too small is reported (CF_E_TOO_LARGE) instead of overwriting a neighbour.
 // ------------------------------------------------------------------------------------------------
-static const uint32_t SUB_MAX_RULES = 32;
+static const uint32_t SUB_LAUNCH_RULES = 32;    // rules per sub_kernel launch; longer programs continue in further launches
 static const uint32_t SUB_WIN = 512;            // start positions examined per warp iteration
 static const uint32_t SUB_WARPS = 4;
+static const uint64_t SUB_OVERFLOW = ~1ull;     // rec[0] of a unit whose output outgrew its scratch bound (rec[1] = the rule)
 
 struct SubRule {
   cf::DfaTables dfa;
@@ -600,23 +602,27 @@ struct SubParams {
   const uint64_t* soff;       // per selected unit: offset of its scratch area (two buffers of `bound` bytes)
   const uint64_t* bound;
   uint8_t* scratch;
-  uint64_t* rec;              // per selected unit: [0] = final text offset in scratch (or ~0: unchanged), [1] = length
+  uint64_t* rec;              // per selected unit: [0] = text offset in scratch (~0: unchanged, SUB_OVERFLOW), [1] = length
   uint32_t* pike;             // per selected unit: pike_words of Pike-VM scratch (rules with group references only)
   uint64_t pike_words;
   uint32_t n_sel;
   uint32_t n_rules;
-  SubRule rules[SUB_MAX_RULES];
+  uint32_t first_rule;        // program index of rules[0]
+  uint32_t resume;            // 0: start from the stream; 1: continue from `rec` (a previous launch's rules)
+  SubRule rules[SUB_LAUNCH_RULES];
 };
 
-__device__ __forceinline__ void warp_copy(uint8_t* dst, const uint8_t* src, uint64_t n, uint32_t lane) {
-  for (uint64_t i = lane; i < n; i += 32) dst[i] = src[i];
+// dst[pos, pos + n) = src[0, n), clamped to dst[0, cap): an output longer than its scratch area never reaches a neighbour's
+__device__ __forceinline__ void warp_put(uint8_t* dst, uint64_t pos, uint64_t cap, const uint8_t* src, uint64_t n, uint32_t lane) {
+  const uint64_t m = pos < cap ? (n < cap - pos ? n : cap - pos) : 0;
+  for (uint64_t i = lane; i < m; i += 32) dst[pos + i] = src[i];
 }
 
-// One replacement at out_pos for the match of rule R that starts at sp: the literal, or the template with the group texts of
-// THIS match (captures by lane 0's Pike VM pass, spans broadcast through shared memory).  Returns the bytes written.
+// One replacement at dst[pos] (clamped to cap) for the match of rule R that starts at sp: the literal, or the template with the group
+// texts of THIS match (captures by lane 0's Pike VM pass, spans broadcast through shared memory).  Returns the length of the replacement.
 __device__ __forceinline__ uint64_t emit_replacement(const SubRule& R, const uint8_t* src, uint64_t len, uint64_t sp, bool must_advance, uint8_t* dst,
-                                                     uint32_t lane, uint32_t* caps_s, uint32_t* pike) {
-  if (R.n_parts == 0) { warp_copy(dst, R.repl, R.repl_len, lane); return R.repl_len; }
+                                                     uint64_t pos, uint64_t cap, uint32_t lane, uint32_t* caps_s, uint32_t* pike) {
+  if (R.n_parts == 0) { warp_put(dst, pos, cap, R.repl, R.repl_len, lane); return R.repl_len; }
   __syncwarp();
   if (lane == 0) {
     for (uint32_t k = 0; k < R.nfa.nslots; ++k) caps_s[k] = cf::CAP_UNSET;
@@ -626,10 +632,10 @@ __device__ __forceinline__ uint64_t emit_replacement(const SubRule& R, const uin
   uint64_t o = 0;
   for (uint32_t k = 0; k < R.n_parts; ++k) {
     const uint32_t kind = R.parts[3 * k], a = R.parts[3 * k + 1], b = R.parts[3 * k + 2];
-    if (kind == 0) { warp_copy(dst + o, R.repl + a, b, lane); o += b; }
+    if (kind == 0) { warp_put(dst, pos + o, cap, R.repl + a, b, lane); o += b; }
     else {
       const uint32_t g0 = caps_s[2 * a], g1 = caps_s[2 * a + 1];
-      if (g0 != cf::CAP_UNSET && g1 != cf::CAP_UNSET && g1 >= g0) { warp_copy(dst + o, src + g0, g1 - g0, lane); o += g1 - g0; }
+      if (g0 != cf::CAP_UNSET && g1 != cf::CAP_UNSET && g1 >= g0) { warp_put(dst, pos + o, cap, src + g0, g1 - g0, lane); o += g1 - g0; }
     }
   }
   return o;
@@ -647,9 +653,20 @@ __global__ void __launch_bounds__(SUB_WARPS * 32) sub_kernel(const __grid_consta
   const uint32_t u = P.sel[w];
   const uint8_t* src = P.stream + P.offsets[u];
   uint64_t len = P.offsets[u + 1] - P.offsets[u] - 1;
-  uint8_t* bufs[2] = {P.scratch + P.soff[w], P.scratch + P.soff[w] + P.bound[w]};
+  const uint64_t cap = P.bound[w];                          // bytes of each buffer of the pair: every write is clamped to it
+  uint8_t* bufs[2] = {P.scratch + P.soff[w], P.scratch + P.soff[w] + cap};
   uint32_t which = 0;
   bool changed = false;
+  if (P.resume) {          // continue from the previous launch: the stream, or the buffer of the pair it wrote last
+    const uint64_t at = P.rec[2 * (uint64_t)w];
+    if (at == SUB_OVERFLOW) return;
+    if (at != ~0ull) {
+      src = P.scratch + at;
+      len = P.rec[2 * (uint64_t)w + 1];
+      which = src == bufs[0] ? 1 : 0;
+      changed = true;
+    }
+  }
 
   for (uint32_t r = 0; r < P.n_rules; ++r) {
     const SubRule& R = P.rules[r];
@@ -686,12 +703,12 @@ __global__ void __launch_bounds__(SUB_WARPS * 32) sub_kernel(const __grid_consta
             const uint64_t sp = wbase + (uint64_t)L * 8 + k;
             if (sp < cur) continue;                     // inside the previous match
             const uint32_t m1 = mlen[L * 8 + k], m2 = mlen2[L * 8 + k];
-            warp_copy(dst + out_pos, src + copied, sp - copied, lane);
+            warp_put(dst, out_pos, cap, src + copied, sp - copied, lane);
             out_pos += sp - copied;
-            out_pos += emit_replacement(R, src, len, sp, false, dst + out_pos, lane, caps_s, pike);
+            out_pos += emit_replacement(R, src, len, sp, false, dst, out_pos, cap, lane, caps_s, pike);
             ++nmatch;
             if (m1 == 0 && m2) {                        // empty match, then the non-empty one at the same position
-              out_pos += emit_replacement(R, src, len, sp, true, dst + out_pos, lane, caps_s, pike);
+              out_pos += emit_replacement(R, src, len, sp, true, dst, out_pos, cap, lane, caps_s, pike);
               ++nmatch;
             }
             copied = cur = sp + (m1 ? m1 : m2);
@@ -730,9 +747,9 @@ __global__ void __launch_bounds__(SUB_WARPS * 32) sub_kernel(const __grid_consta
           const uint64_t sp = wbase + (uint64_t)L * 16 + k;
           if (sp < cur) continue;                       // inside the previous match
           const uint32_t ml = mlen[L * 16 + k];
-          warp_copy(dst + out_pos, src + copied, sp - copied, lane);
+          warp_put(dst, out_pos, cap, src + copied, sp - copied, lane);
           out_pos += sp - copied;
-          out_pos += emit_replacement(R, src, len, sp, false, dst + out_pos, lane, caps_s, pike);
+          out_pos += emit_replacement(R, src, len, sp, false, dst, out_pos, cap, lane, caps_s, pike);
           copied = cur = sp + ml;
           ++nmatch;
         }
@@ -740,8 +757,12 @@ __global__ void __launch_bounds__(SUB_WARPS * 32) sub_kernel(const __grid_consta
       __syncwarp();
     }
     if (nmatch) {
-      warp_copy(dst + out_pos, src + copied, len - copied, lane);
+      warp_put(dst, out_pos, cap, src + copied, len - copied, lane);
       out_pos += len - copied;
+      if (out_pos > cap) {           // the scratch bound was too small for this rule's output: the host reports the unit and the rule
+        if (lane == 0) { P.rec[2 * (uint64_t)w] = SUB_OVERFLOW; P.rec[2 * (uint64_t)w + 1] = P.first_rule + r; }
+        return;
+      }
       __syncwarp();
       __threadfence_block();
       src = dst;
@@ -750,6 +771,7 @@ __global__ void __launch_bounds__(SUB_WARPS * 32) sub_kernel(const __grid_consta
       changed = true;
     }
   }
+  __syncwarp();                      // every lane has read this unit's `rec` (resume) before lane 0 rewrites it
   if (lane == 0) {
     P.rec[2 * (uint64_t)w] = changed ? (uint64_t)(src - P.scratch) : ~0ull;
     P.rec[2 * (uint64_t)w + 1] = len;
@@ -1086,7 +1108,7 @@ int cf_sub_host(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint32_t* units, uin
                 uint64_t out_cap, uint64_t* out_offsets, uint64_t* out_needed) {
   if (!ctx || !p || !b || !units || !n_sel || !out_offsets) return CF_E_BADARG;
   const uint32_t nr = (uint32_t)p->ordered.size();
-  if (nr == 0 || nr > SUB_MAX_RULES) { ctx->err = "program has no (or too many) substitution rules"; return CF_E_BADARG; }
+  if (nr == 0) { ctx->err = "program has no substitution rules"; return CF_E_BADARG; }
   if (p->h_offsets_owner != b || p->h_offsets_gen != b->generation || p->h_offsets.size() != (size_t)b->n + 1) {
     // unit lengths are needed on the host to size the scratch area
     p->h_offsets.resize((size_t)b->n + 1);
@@ -1094,10 +1116,15 @@ int cf_sub_host(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint32_t* units, uin
     p->h_offsets_owner = b;
     p->h_offsets_gen = b->generation;
   }
-  // worst-case growth of one unit through all rules: a rule with matches of >= ml bytes turns L bytes into at most L * ceil(repl / ml);
-  // a rule that can match "" has at most L + 1 empty and L non-empty matches
+  // Scratch: two buffers of bound[i] bytes per selected unit.  worst[i] = the unit's worst-case growth through all rules: a rule with
+  // matches of >= ml characters (so >= ml bytes) turns L bytes into at most L * ceil(repl / ml); a rule that can match "" has at most
+  // L + 1 empty and L non-empty matches.  Over a long program that product is far above what any text needs (a -> bb, bb -> c, ...
+  // doubles it at every other rule), so the first pass gives a unit at most 64 L + 64 KiB.  The kernel clamps every write to the
+  // unit's bound and reports a unit whose output outgrew it; that unit runs again with 8x the room, up to worst[i].  Outgrowing
+  // worst[i] itself is an internal error (CF_E_TOO_LARGE), never a write into a neighbour's scratch.
+  std::vector<double> worst(n_sel);
   std::vector<uint64_t> soff(n_sel), bound(n_sel);
-  uint64_t total = 0;
+  auto round16 = [](double x) { return ((uint64_t)x + 15) & ~15ull; };
   for (uint32_t i = 0; i < n_sel; ++i) {
     if (units[i] >= b->n) { ctx->err = "unit index out of range"; return CF_E_BADARG; }
     uint64_t len = p->h_offsets[units[i] + 1] - p->h_offsets[units[i]] - 1;
@@ -1111,13 +1138,9 @@ int cf_sub_host(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint32_t* units, uin
       } else if (ml == 0) bd += (2.0 * bd + 1.0) * (double)p->repl_len[r];
       else { const double g = (double)((p->repl_len[r] + ml - 1) / ml); if (g > 1.0) bd *= g; }
     }
-    bd += 16.0;
-    if (bd > 4e9) { ctx->err = "substitution rules expand a unit beyond 4 GB"; return CF_E_CAPACITY; }
-    bound[i] = ((uint64_t)bd + 15) & ~15ull;
-    soff[i] = total;
-    total += 2 * bound[i];
+    worst[i] = bd + 16.0;
+    bound[i] = round16(std::min(worst[i], 64.0 * (double)len + 65536.0));
   }
-  if (total > (8ull << 30)) { ctx->err = "substitution scratch exceeds 8 GiB"; return CF_E_CAPACITY; }
   uint8_t* d_scratch = nullptr;
   uint32_t* d_sel = nullptr;
   uint64_t *d_soff = nullptr, *d_bound = nullptr, *d_rec = nullptr, *d_ooff = nullptr;
@@ -1127,31 +1150,17 @@ int cf_sub_host(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint32_t* units, uin
   do {
 #define SUB_CUDA(call) { cudaError_t e_ = (call); if (e_ != cudaSuccess) { ctx->err = std::string(#call) + ": " + cudaGetErrorString(e_); rc = CF_E_CUDA; break; } }
     // grow-only scratch of the context: no cudaMalloc / cudaFree per call
-    if ((rc = cf_dev_reserve(ctx, ctx->tmp[8], total ? total : 16)) || (rc = cf_dev_reserve(ctx, ctx->tmp[9], (size_t)n_sel * 4)) ||
+    if ((rc = cf_dev_reserve(ctx, ctx->tmp[9], (size_t)n_sel * 4)) ||
         (rc = cf_dev_reserve(ctx, ctx->tmp[10], (size_t)n_sel * 8)) || (rc = cf_dev_reserve(ctx, ctx->tmp[11], (size_t)n_sel * 8)) ||
         (rc = cf_dev_reserve(ctx, ctx->tmp[12], (size_t)n_sel * 16)) || (rc = cf_dev_reserve(ctx, ctx->tmp[13], ((size_t)n_sel + 1) * 8))) break;
-    d_scratch = (uint8_t*)ctx->tmp[8].p; d_sel = (uint32_t*)ctx->tmp[9].p; d_soff = (uint64_t*)ctx->tmp[10].p; d_bound = (uint64_t*)ctx->tmp[11].p;
+    d_sel = (uint32_t*)ctx->tmp[9].p; d_soff = (uint64_t*)ctx->tmp[10].p; d_bound = (uint64_t*)ctx->tmp[11].p;
     d_rec = (uint64_t*)ctx->tmp[12].p; d_ooff = (uint64_t*)ctx->tmp[13].p;
     SUB_CUDA(cudaMemcpy(d_sel, units, n_sel * 4, cudaMemcpyHostToDevice));
-    SUB_CUDA(cudaMemcpy(d_soff, soff.data(), n_sel * 8, cudaMemcpyHostToDevice));
-    SUB_CUDA(cudaMemcpy(d_bound, bound.data(), n_sel * 8, cudaMemcpyHostToDevice));
     SubParams SP;
     SP.stream = b->d_buf + cf::FRONT_PAD;
     SP.offsets = b->d_offsets;
-    SP.sel = d_sel; SP.soff = d_soff; SP.bound = d_bound; SP.scratch = d_scratch; SP.rec = d_rec;
-    SP.n_sel = n_sel; SP.n_rules = nr;
-    for (uint32_t r = 0; r < nr; ++r) {
-      SP.rules[r].dfa = p->ordered[r].t;
-      SP.rules[r].E = p->d_ordered_E[r];
-      SP.rules[r].repl = p->d_repl[r];
-      SP.rules[r].repl_len = p->repl_len[r];
-      SP.rules[r].nullable = p->ordered_minlen[r] == 0;
-      const cf_prog::RuleTmpl& T = p->tmpl[r];
-      SP.rules[r].parts = T.d_parts;
-      SP.rules[r].n_parts = T.n_parts;
-      SP.rules[r].nfa.code = T.d_code; SP.rules[r].nfa.setbits = T.d_sets;
-      SP.rules[r].nfa.ninst = T.ninst; SP.rules[r].nfa.start = 0; SP.rules[r].nfa.wpc = T.wpc; SP.rules[r].nfa.nslots = T.nslots;
-    }
+    SP.sel = d_sel; SP.soff = d_soff; SP.bound = d_bound; SP.rec = d_rec;
+    SP.n_sel = n_sel;
     SP.pike = nullptr; SP.pike_words = 0;
     for (uint32_t r = 0; r < nr; ++r)
       if (p->tmpl[r].n_parts) { const uint64_t wds = cf::pike_scratch_words(p->tmpl[r].ninst, p->tmpl[r].nslots); if (wds > SP.pike_words) SP.pike_words = wds; }
@@ -1160,10 +1169,58 @@ int cf_sub_host(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint32_t* units, uin
       if ((rc = cf_dev_reserve(ctx, ctx->tmp[15], (size_t)n_sel * SP.pike_words * 4))) break;
       SP.pike = (uint32_t*)ctx->tmp[15].p;
     }
-    sub_kernel<<<(n_sel + SUB_WARPS - 1) / SUB_WARPS, SUB_WARPS * 32>>>(SP);
-    ctx->launches++;
-    SUB_CUDA(cudaGetLastError());
-    SUB_CUDA(cudaMemcpy(rec.data(), d_rec, n_sel * 16, cudaMemcpyDeviceToHost));
+    for (bool again = true; again;) {        // one pass, and another while some unit outgrew a bound below its worst case
+      again = false;
+      uint64_t total = 0;
+      for (uint32_t i = 0; i < n_sel; ++i) { soff[i] = total; total += 2 * bound[i]; }
+      if (total > (8ull << 30)) { ctx->err = "substitution scratch exceeds 8 GiB"; rc = CF_E_CAPACITY; break; }
+      if ((rc = cf_dev_reserve(ctx, ctx->tmp[8], total))) break;
+      d_scratch = SP.scratch = (uint8_t*)ctx->tmp[8].p;
+      SUB_CUDA(cudaMemcpy(d_soff, soff.data(), n_sel * 8, cudaMemcpyHostToDevice));
+      SUB_CUDA(cudaMemcpy(d_bound, bound.data(), n_sel * 8, cudaMemcpyHostToDevice));
+      // SUB_LAUNCH_RULES rules per launch; each further launch continues every unit from the record the previous one left
+      for (uint32_t r0 = 0; r0 < nr; r0 += SUB_LAUNCH_RULES) {
+        SP.first_rule = r0;
+        SP.resume = r0 > 0;
+        SP.n_rules = std::min(nr - r0, SUB_LAUNCH_RULES);
+        for (uint32_t i = 0; i < SP.n_rules; ++i) {
+          const uint32_t r = r0 + i;
+          SubRule& S = SP.rules[i];
+          S.dfa = p->ordered[r].t;
+          S.E = p->d_ordered_E[r];
+          S.repl = p->d_repl[r];
+          S.repl_len = p->repl_len[r];
+          S.nullable = p->ordered_minlen[r] == 0;
+          const cf_prog::RuleTmpl& T = p->tmpl[r];
+          S.parts = T.d_parts;
+          S.n_parts = T.n_parts;
+          S.nfa.code = T.d_code; S.nfa.setbits = T.d_sets;
+          S.nfa.ninst = T.ninst; S.nfa.start = 0; S.nfa.wpc = T.wpc; S.nfa.nslots = T.nslots;
+        }
+        sub_kernel<<<(n_sel + SUB_WARPS - 1) / SUB_WARPS, SUB_WARPS * 32>>>(SP);
+        ctx->launches++;
+        SUB_CUDA(cudaGetLastError());
+      }
+      if (rc) break;
+      SUB_CUDA(cudaMemcpy(rec.data(), d_rec, n_sel * 16, cudaMemcpyDeviceToHost));
+      for (uint32_t i = 0; i < n_sel && !rc; ++i) {
+        if (rec[2 * (size_t)i] != SUB_OVERFLOW) continue;
+        const double grown = std::min(worst[i], 8.0 * (double)bound[i]);
+        if ((double)bound[i] >= worst[i]) {
+          ctx->err = "substitution of unit " + std::to_string(units[i]) + " (selection index " + std::to_string(i) + "): the output of rule " +
+                     std::to_string(rec[2 * (size_t)i + 1]) + " exceeds the worst-case bound of its scratch";
+          rc = CF_E_TOO_LARGE;
+        } else if (grown > 4e9) {
+          ctx->err = "substitution rules expand a unit beyond 4 GB";
+          rc = CF_E_CAPACITY;
+        } else {
+          bound[i] = round16(grown);
+          again = true;
+        }
+      }
+      if (rc) break;
+    }
+    if (rc) break;
     uint64_t need = 0;
     for (uint32_t i = 0; i < n_sel; ++i) { out_offsets[i] = need; need += rec[2 * (size_t)i + 1]; }
     out_offsets[n_sel] = need;
