@@ -38,6 +38,9 @@ struct cf_ctx {
   size_t h_stage_bytes = 0;
   const uint8_t* run_out = nullptr;   // device buffer of the last CF_RUN_OUTPUTS_RESIDENT call
   uint64_t run_out_bytes = 0;
+  // cf_run_batch: the substitution runs on `side` (non-blocking, highest priority) beside the TOON kernel on the legacy stream
+  cudaStream_t side = nullptr;
+  cudaEvent_t ev_scan = nullptr, ev_toon = nullptr, ev_sub = nullptr;
   // optional per-launch timing of the dominant kernel (bench.py roofline): event pairs
   std::vector<cudaEvent_t> prof_ev;
   uint32_t prof_used = 0;
@@ -112,6 +115,14 @@ struct cf_batch {
 // grow-only device / pinned-host scratch of the *_host entry points (defined in cfjson.cu)
 int cf_dev_reserve(cf_ctx* ctx, cf_ctx::DevBuf& b, size_t need);
 int cf_stage_reserve(cf_ctx* ctx, size_t need);
+
+// regex_filter substitution of the selected units on stream `st` (cfgpu.cu); the rewritten texts stay on the device.  Unit units[i]
+// ends as rec[2i+1] bytes at ctx->tmp[8] + rec[2i], or as the unit itself in the batch's stream when rec[2i] == ~0 (no rule changed
+// it).  h_offsets: host copy of the batch's offsets (scratch sizing); h_stage: pinned, cf_sub_stage_bytes(n_sel) bytes, and *rec
+// points into it.  Returns with the work on `st` done.  Only the scratch tmp[8..15] is written.
+size_t cf_sub_stage_bytes(uint32_t n_sel);
+int cf_sub_device(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint64_t* h_offsets, const uint32_t* units, uint32_t n_sel, cudaStream_t st,
+                  uint8_t* h_stage, const uint64_t** rec);
 
 // sequential JSON kernels (cfjson_seq.cu)
 namespace cfj { struct JNode; }

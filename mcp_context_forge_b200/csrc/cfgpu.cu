@@ -826,6 +826,113 @@ static int upload_dfa(cf_ctx* ctx, const cfre::DfaOut& d, DevDfa& o) {
   return CF_OK;
 }
 
+// ---- the substitution pass shared by cf_sub_host and cf_run_batch (cf_internal.h)
+// Descriptors of a pass, one H2D from pinned staging into tmp[9]: soff[n] | bound[n] | sel[n]; then rec[2n] comes back in one D2H.
+static size_t sub_desc_bytes(uint32_t n) { return ((size_t)n * 20 + 15) & ~(size_t)15; }
+static const uint32_t* sub_desc_sel(const cf_ctx* ctx, uint32_t n) { return (const uint32_t*)((const uint64_t*)ctx->tmp[9].p + 2 * (size_t)n); }
+size_t cf_sub_stage_bytes(uint32_t n_sel) { return sub_desc_bytes(n_sel) + (size_t)n_sel * 16; }
+
+int cf_sub_device(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint64_t* h_offsets, const uint32_t* units, uint32_t n_sel, cudaStream_t st,
+                  uint8_t* h_stage, const uint64_t** rec_out) {
+  const uint32_t nr = (uint32_t)p->ordered.size();
+  if (nr == 0) { ctx->err = "program has no substitution rules"; return CF_E_BADARG; }
+  uint64_t* soff = (uint64_t*)h_stage;
+  uint64_t* bound = soff + n_sel;
+  uint32_t* sel = (uint32_t*)(bound + n_sel);
+  uint64_t* rec = (uint64_t*)(h_stage + sub_desc_bytes(n_sel));
+  // Scratch: two buffers of bound[i] bytes per selected unit.  worst[i] = the unit's worst-case growth through all rules: a rule with
+  // matches of >= ml characters (so >= ml bytes) turns L bytes into at most L * ceil(repl / ml); a rule that can match "" has at most
+  // L + 1 empty and L non-empty matches.  Over a long program that product is far above what any text needs (a -> bb, bb -> c, ...
+  // doubles it at every other rule), so the first pass gives a unit at most 64 L + 64 KiB.  The kernel clamps every write to the
+  // unit's bound and reports a unit whose output outgrew it; that unit runs again with 8x the room, up to worst[i].  Outgrowing
+  // worst[i] itself is an internal error (CF_E_TOO_LARGE), never a write into a neighbour's scratch.
+  std::vector<double> worst(n_sel);
+  auto round16 = [](double x) { return ((uint64_t)x + 15) & ~15ull; };
+  for (uint32_t i = 0; i < n_sel; ++i) {
+    if (units[i] >= b->n) { ctx->err = "unit index out of range"; return CF_E_BADARG; }
+    sel[i] = units[i];
+    uint64_t len = h_offsets[units[i] + 1] - h_offsets[units[i]] - 1;
+    double bd = (double)len;
+    for (uint32_t r = 0; r < nr; ++r) {
+      const uint32_t ml = p->ordered_minlen[r];
+      const cf_prog::RuleTmpl& T = p->tmpl[r];
+      if (T.n_parts) {             // every match: its literals + each referenced group (at most the match itself)
+        const double nmatch = ml ? bd / ml + 1.0 : 2.0 * bd + 1.0;
+        bd = bd * (1.0 + T.nrefs) + nmatch * (double)T.lit_len;
+      } else if (ml == 0) bd += (2.0 * bd + 1.0) * (double)p->repl_len[r];
+      else { const double g = (double)((p->repl_len[r] + ml - 1) / ml); if (g > 1.0) bd *= g; }
+    }
+    worst[i] = bd + 16.0;
+    bound[i] = round16(std::min(worst[i], 64.0 * (double)len + 65536.0));
+  }
+  int rc;
+  // grow-only scratch of the context: no cudaMalloc / cudaFree per call
+  if ((rc = cf_dev_reserve(ctx, ctx->tmp[9], sub_desc_bytes(n_sel))) || (rc = cf_dev_reserve(ctx, ctx->tmp[12], (size_t)n_sel * 16))) return rc;
+  uint64_t* d_desc = (uint64_t*)ctx->tmp[9].p;
+  SubParams SP;
+  SP.stream = b->d_buf + cf::FRONT_PAD;
+  SP.offsets = b->d_offsets;
+  SP.soff = d_desc; SP.bound = d_desc + n_sel; SP.sel = sub_desc_sel(ctx, n_sel);
+  SP.rec = (uint64_t*)ctx->tmp[12].p;
+  SP.n_sel = n_sel;
+  SP.pike = nullptr; SP.pike_words = 0;
+  for (uint32_t r = 0; r < nr; ++r)
+    if (p->tmpl[r].n_parts) { const uint64_t wds = cf::pike_scratch_words(p->tmpl[r].ninst, p->tmpl[r].nslots); if (wds > SP.pike_words) SP.pike_words = wds; }
+  if (SP.pike_words) {
+    if ((uint64_t)n_sel * SP.pike_words * 4 > (4ull << 30)) { ctx->err = "capture scratch exceeds 4 GiB (too many units for a rule with group references)"; return CF_E_CAPACITY; }
+    if ((rc = cf_dev_reserve(ctx, ctx->tmp[15], (size_t)n_sel * SP.pike_words * 4))) return rc;
+    SP.pike = (uint32_t*)ctx->tmp[15].p;
+  }
+  for (bool again = true; again;) {        // one pass, and another while some unit outgrew a bound below its worst case
+    again = false;
+    uint64_t total = 0;
+    for (uint32_t i = 0; i < n_sel; ++i) { soff[i] = total; total += 2 * bound[i]; }
+    if (total > (8ull << 30)) { ctx->err = "substitution scratch exceeds 8 GiB"; return CF_E_CAPACITY; }
+    if ((rc = cf_dev_reserve(ctx, ctx->tmp[8], total))) return rc;
+    SP.scratch = (uint8_t*)ctx->tmp[8].p;
+    CF_CUDA(ctx, cudaMemcpyAsync(d_desc, h_stage, sub_desc_bytes(n_sel), cudaMemcpyHostToDevice, st));
+    // SUB_LAUNCH_RULES rules per launch; each further launch continues every unit from the record the previous one left
+    for (uint32_t r0 = 0; r0 < nr; r0 += SUB_LAUNCH_RULES) {
+      SP.first_rule = r0;
+      SP.resume = r0 > 0;
+      SP.n_rules = std::min(nr - r0, SUB_LAUNCH_RULES);
+      for (uint32_t i = 0; i < SP.n_rules; ++i) {
+        const uint32_t r = r0 + i;
+        SubRule& S = SP.rules[i];
+        S.dfa = p->ordered[r].t;
+        S.E = p->d_ordered_E[r];
+        S.repl = p->d_repl[r];
+        S.repl_len = p->repl_len[r];
+        S.nullable = p->ordered_minlen[r] == 0;
+        const cf_prog::RuleTmpl& T = p->tmpl[r];
+        S.parts = T.d_parts;
+        S.n_parts = T.n_parts;
+        S.nfa.code = T.d_code; S.nfa.setbits = T.d_sets;
+        S.nfa.ninst = T.ninst; S.nfa.start = 0; S.nfa.wpc = T.wpc; S.nfa.nslots = T.nslots;
+      }
+      sub_kernel<<<(n_sel + SUB_WARPS - 1) / SUB_WARPS, SUB_WARPS * 32, 0, st>>>(SP);
+      ctx->launches++;
+      CF_CUDA(ctx, cudaGetLastError());
+    }
+    CF_CUDA(ctx, cudaMemcpyAsync(rec, SP.rec, (size_t)n_sel * 16, cudaMemcpyDeviceToHost, st));
+    CF_CUDA(ctx, cudaStreamSynchronize(st));
+    for (uint32_t i = 0; i < n_sel; ++i) {
+      if (rec[2 * (size_t)i] != SUB_OVERFLOW) continue;
+      const double grown = std::min(worst[i], 8.0 * (double)bound[i]);
+      if ((double)bound[i] >= worst[i]) {
+        ctx->err = "substitution of unit " + std::to_string(units[i]) + " (selection index " + std::to_string(i) + "): the output of rule " +
+                   std::to_string(rec[2 * (size_t)i + 1]) + " exceeds the worst-case bound of its scratch";
+        return CF_E_TOO_LARGE;
+      }
+      if (grown > 4e9) { ctx->err = "substitution rules expand a unit beyond 4 GB"; return CF_E_CAPACITY; }
+      bound[i] = round16(grown);
+      again = true;
+    }
+  }
+  *rec_out = rec;
+  return CF_OK;
+}
+
 extern "C" {
 
 int cf_init(int device_ordinal, cf_ctx** out) {
@@ -844,6 +951,10 @@ int cf_init(int device_ordinal, cf_ctx** out) {
   CF_CUDA(ctx, cudaMalloc(&ctx->d_qstate, 4 * sizeof(uint64_t)));
   CF_CUDA(ctx, cudaMemset(ctx->d_qstate, 0, 4 * sizeof(uint64_t)));
   CF_CUDA(ctx, cudaMalloc(&ctx->d_queue, (size_t)ctx->qcap * sizeof(uint64_t)));
+  int prio_lo = 0, prio_hi = 0;   // the few substitution blocks take SMs as TOON blocks retire instead of queueing behind all of them
+  CF_CUDA(ctx, cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
+  CF_CUDA(ctx, cudaStreamCreateWithPriority(&ctx->side, cudaStreamNonBlocking, prio_hi));
+  for (cudaEvent_t* e : {&ctx->ev_scan, &ctx->ev_toon, &ctx->ev_sub}) CF_CUDA(ctx, cudaEventCreateWithFlags(e, cudaEventDisableTiming));
   if (const char* e = getenv("CF_SCAN_WARPS")) ctx->scan_warps = (uint32_t)atoi(e);
   if (const char* e = getenv("CF_SCAN_ACC")) ctx->scan_acc = (uint32_t)atoi(e);
   if (const char* e = getenv("CF_SCAN_LB")) ctx->scan_lane_bytes = (uint32_t)atoi(e);
@@ -866,6 +977,8 @@ void cf_shutdown(cf_ctx* ctx) {
   for (auto& t : ctx->tmp) cudaFree(t.p);
   cudaFree(ctx->d_tok.p); cudaFree(ctx->d_ntok.p);
   if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
+  if (ctx->side) cudaStreamDestroy(ctx->side);
+  for (cudaEvent_t e : {ctx->ev_scan, ctx->ev_toon, ctx->ev_sub}) if (e) cudaEventDestroy(e);
   delete ctx;
 }
 
@@ -1107,8 +1220,7 @@ int cf_scan_host(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint8_t* stream, ui
 int cf_sub_host(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint32_t* units, uint32_t n_sel, uint8_t* out_bytes,
                 uint64_t out_cap, uint64_t* out_offsets, uint64_t* out_needed) {
   if (!ctx || !p || !b || !units || !n_sel || !out_offsets) return CF_E_BADARG;
-  const uint32_t nr = (uint32_t)p->ordered.size();
-  if (nr == 0) { ctx->err = "program has no substitution rules"; return CF_E_BADARG; }
+  if (p->ordered.empty()) { ctx->err = "program has no substitution rules"; return CF_E_BADARG; }
   if (p->h_offsets_owner != b || p->h_offsets_gen != b->generation || p->h_offsets.size() != (size_t)b->n + 1) {
     // unit lengths are needed on the host to size the scratch area
     p->h_offsets.resize((size_t)b->n + 1);
@@ -1116,128 +1228,27 @@ int cf_sub_host(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint32_t* units, uin
     p->h_offsets_owner = b;
     p->h_offsets_gen = b->generation;
   }
-  // Scratch: two buffers of bound[i] bytes per selected unit.  worst[i] = the unit's worst-case growth through all rules: a rule with
-  // matches of >= ml characters (so >= ml bytes) turns L bytes into at most L * ceil(repl / ml); a rule that can match "" has at most
-  // L + 1 empty and L non-empty matches.  Over a long program that product is far above what any text needs (a -> bb, bb -> c, ...
-  // doubles it at every other rule), so the first pass gives a unit at most 64 L + 64 KiB.  The kernel clamps every write to the
-  // unit's bound and reports a unit whose output outgrew it; that unit runs again with 8x the room, up to worst[i].  Outgrowing
-  // worst[i] itself is an internal error (CF_E_TOO_LARGE), never a write into a neighbour's scratch.
-  std::vector<double> worst(n_sel);
-  std::vector<uint64_t> soff(n_sel), bound(n_sel);
-  auto round16 = [](double x) { return ((uint64_t)x + 15) & ~15ull; };
-  for (uint32_t i = 0; i < n_sel; ++i) {
-    if (units[i] >= b->n) { ctx->err = "unit index out of range"; return CF_E_BADARG; }
-    uint64_t len = p->h_offsets[units[i] + 1] - p->h_offsets[units[i]] - 1;
-    double bd = (double)len;
-    for (uint32_t r = 0; r < nr; ++r) {
-      const uint32_t ml = p->ordered_minlen[r];
-      const cf_prog::RuleTmpl& T = p->tmpl[r];
-      if (T.n_parts) {             // every match: its literals + each referenced group (at most the match itself)
-        const double nmatch = ml ? bd / ml + 1.0 : 2.0 * bd + 1.0;
-        bd = bd * (1.0 + T.nrefs) + nmatch * (double)T.lit_len;
-      } else if (ml == 0) bd += (2.0 * bd + 1.0) * (double)p->repl_len[r];
-      else { const double g = (double)((p->repl_len[r] + ml - 1) / ml); if (g > 1.0) bd *= g; }
-    }
-    worst[i] = bd + 16.0;
-    bound[i] = round16(std::min(worst[i], 64.0 * (double)len + 65536.0));
+  int rc;
+  if ((rc = cf_stage_reserve(ctx, cf_sub_stage_bytes(n_sel)))) return rc;
+  const uint64_t* rec = nullptr;
+  if ((rc = cf_sub_device(ctx, p, b, p->h_offsets.data(), units, n_sel, 0, (uint8_t*)ctx->h_stage, &rec))) return rc;
+  uint64_t need = 0;
+  for (uint32_t i = 0; i < n_sel; ++i) { out_offsets[i] = need; need += rec[2 * (size_t)i + 1]; }
+  out_offsets[n_sel] = need;
+  if (out_needed) *out_needed = need;
+  if (need > out_cap || (!out_bytes && need)) { ctx->err = "output buffer too small"; return CF_E_CAPACITY; }
+  if (need) {
+    if ((rc = cf_dev_reserve(ctx, ctx->tmp[13], ((size_t)n_sel + 1) * 8)) || (rc = cf_dev_reserve(ctx, ctx->tmp[14], need))) return rc;
+    uint64_t* d_ooff = (uint64_t*)ctx->tmp[13].p;
+    uint8_t* d_out = (uint8_t*)ctx->tmp[14].p;
+    CF_CUDA(ctx, cudaMemcpy(d_ooff, out_offsets, ((size_t)n_sel + 1) * 8, cudaMemcpyHostToDevice));
+    sub_compact_kernel<<<n_sel, 256>>>(b->d_buf + cf::FRONT_PAD, b->d_offsets, sub_desc_sel(ctx, n_sel), (const uint8_t*)ctx->tmp[8].p,
+                                       (const uint64_t*)ctx->tmp[12].p, d_ooff, d_out, n_sel);
+    ctx->launches++;
+    CF_CUDA(ctx, cudaGetLastError());
+    CF_CUDA(ctx, cudaMemcpy(out_bytes, d_out, need, cudaMemcpyDeviceToHost));
   }
-  uint8_t* d_scratch = nullptr;
-  uint32_t* d_sel = nullptr;
-  uint64_t *d_soff = nullptr, *d_bound = nullptr, *d_rec = nullptr, *d_ooff = nullptr;
-  uint8_t* d_out = nullptr;
-  int rc = CF_OK;
-  std::vector<uint64_t> rec(2 * (size_t)n_sel);
-  do {
-#define SUB_CUDA(call) { cudaError_t e_ = (call); if (e_ != cudaSuccess) { ctx->err = std::string(#call) + ": " + cudaGetErrorString(e_); rc = CF_E_CUDA; break; } }
-    // grow-only scratch of the context: no cudaMalloc / cudaFree per call
-    if ((rc = cf_dev_reserve(ctx, ctx->tmp[9], (size_t)n_sel * 4)) ||
-        (rc = cf_dev_reserve(ctx, ctx->tmp[10], (size_t)n_sel * 8)) || (rc = cf_dev_reserve(ctx, ctx->tmp[11], (size_t)n_sel * 8)) ||
-        (rc = cf_dev_reserve(ctx, ctx->tmp[12], (size_t)n_sel * 16)) || (rc = cf_dev_reserve(ctx, ctx->tmp[13], ((size_t)n_sel + 1) * 8))) break;
-    d_sel = (uint32_t*)ctx->tmp[9].p; d_soff = (uint64_t*)ctx->tmp[10].p; d_bound = (uint64_t*)ctx->tmp[11].p;
-    d_rec = (uint64_t*)ctx->tmp[12].p; d_ooff = (uint64_t*)ctx->tmp[13].p;
-    SUB_CUDA(cudaMemcpy(d_sel, units, n_sel * 4, cudaMemcpyHostToDevice));
-    SubParams SP;
-    SP.stream = b->d_buf + cf::FRONT_PAD;
-    SP.offsets = b->d_offsets;
-    SP.sel = d_sel; SP.soff = d_soff; SP.bound = d_bound; SP.rec = d_rec;
-    SP.n_sel = n_sel;
-    SP.pike = nullptr; SP.pike_words = 0;
-    for (uint32_t r = 0; r < nr; ++r)
-      if (p->tmpl[r].n_parts) { const uint64_t wds = cf::pike_scratch_words(p->tmpl[r].ninst, p->tmpl[r].nslots); if (wds > SP.pike_words) SP.pike_words = wds; }
-    if (SP.pike_words) {
-      if ((uint64_t)n_sel * SP.pike_words * 4 > (4ull << 30)) { ctx->err = "capture scratch exceeds 4 GiB (too many units for a rule with group references)"; rc = CF_E_CAPACITY; break; }
-      if ((rc = cf_dev_reserve(ctx, ctx->tmp[15], (size_t)n_sel * SP.pike_words * 4))) break;
-      SP.pike = (uint32_t*)ctx->tmp[15].p;
-    }
-    for (bool again = true; again;) {        // one pass, and another while some unit outgrew a bound below its worst case
-      again = false;
-      uint64_t total = 0;
-      for (uint32_t i = 0; i < n_sel; ++i) { soff[i] = total; total += 2 * bound[i]; }
-      if (total > (8ull << 30)) { ctx->err = "substitution scratch exceeds 8 GiB"; rc = CF_E_CAPACITY; break; }
-      if ((rc = cf_dev_reserve(ctx, ctx->tmp[8], total))) break;
-      d_scratch = SP.scratch = (uint8_t*)ctx->tmp[8].p;
-      SUB_CUDA(cudaMemcpy(d_soff, soff.data(), n_sel * 8, cudaMemcpyHostToDevice));
-      SUB_CUDA(cudaMemcpy(d_bound, bound.data(), n_sel * 8, cudaMemcpyHostToDevice));
-      // SUB_LAUNCH_RULES rules per launch; each further launch continues every unit from the record the previous one left
-      for (uint32_t r0 = 0; r0 < nr; r0 += SUB_LAUNCH_RULES) {
-        SP.first_rule = r0;
-        SP.resume = r0 > 0;
-        SP.n_rules = std::min(nr - r0, SUB_LAUNCH_RULES);
-        for (uint32_t i = 0; i < SP.n_rules; ++i) {
-          const uint32_t r = r0 + i;
-          SubRule& S = SP.rules[i];
-          S.dfa = p->ordered[r].t;
-          S.E = p->d_ordered_E[r];
-          S.repl = p->d_repl[r];
-          S.repl_len = p->repl_len[r];
-          S.nullable = p->ordered_minlen[r] == 0;
-          const cf_prog::RuleTmpl& T = p->tmpl[r];
-          S.parts = T.d_parts;
-          S.n_parts = T.n_parts;
-          S.nfa.code = T.d_code; S.nfa.setbits = T.d_sets;
-          S.nfa.ninst = T.ninst; S.nfa.start = 0; S.nfa.wpc = T.wpc; S.nfa.nslots = T.nslots;
-        }
-        sub_kernel<<<(n_sel + SUB_WARPS - 1) / SUB_WARPS, SUB_WARPS * 32>>>(SP);
-        ctx->launches++;
-        SUB_CUDA(cudaGetLastError());
-      }
-      if (rc) break;
-      SUB_CUDA(cudaMemcpy(rec.data(), d_rec, n_sel * 16, cudaMemcpyDeviceToHost));
-      for (uint32_t i = 0; i < n_sel && !rc; ++i) {
-        if (rec[2 * (size_t)i] != SUB_OVERFLOW) continue;
-        const double grown = std::min(worst[i], 8.0 * (double)bound[i]);
-        if ((double)bound[i] >= worst[i]) {
-          ctx->err = "substitution of unit " + std::to_string(units[i]) + " (selection index " + std::to_string(i) + "): the output of rule " +
-                     std::to_string(rec[2 * (size_t)i + 1]) + " exceeds the worst-case bound of its scratch";
-          rc = CF_E_TOO_LARGE;
-        } else if (grown > 4e9) {
-          ctx->err = "substitution rules expand a unit beyond 4 GB";
-          rc = CF_E_CAPACITY;
-        } else {
-          bound[i] = round16(grown);
-          again = true;
-        }
-      }
-      if (rc) break;
-    }
-    if (rc) break;
-    uint64_t need = 0;
-    for (uint32_t i = 0; i < n_sel; ++i) { out_offsets[i] = need; need += rec[2 * (size_t)i + 1]; }
-    out_offsets[n_sel] = need;
-    if (out_needed) *out_needed = need;
-    if (need > out_cap || (!out_bytes && need)) { ctx->err = "output buffer too small"; rc = CF_E_CAPACITY; break; }
-    if (need) {
-      if ((rc = cf_dev_reserve(ctx, ctx->tmp[14], need))) break;
-      d_out = (uint8_t*)ctx->tmp[14].p;
-      SUB_CUDA(cudaMemcpy(d_ooff, out_offsets, ((size_t)n_sel + 1) * 8, cudaMemcpyHostToDevice));
-      sub_compact_kernel<<<n_sel, 256>>>(b->d_buf + cf::FRONT_PAD, b->d_offsets, d_sel, d_scratch, d_rec, d_ooff, d_out, n_sel);
-      ctx->launches++;
-      SUB_CUDA(cudaGetLastError());
-      SUB_CUDA(cudaMemcpy(out_bytes, d_out, need, cudaMemcpyDeviceToHost));
-    }
-#undef SUB_CUDA
-  } while (0);
-  return rc;
+  return CF_OK;
 }
 
 int cf_profile_begin(cf_ctx* ctx, uint32_t max_launches) {

@@ -365,8 +365,43 @@ int cf_classify_keys_host(cf_ctx* ctx, cf_batch* b, const uint8_t* stream, uint6
 }
 
 
+// gather of every text cf_run_batch produced: dst[out_off[u], out_off[u+1]) = src[u][0, len), one warp per unit.  16-byte stores;
+// 16-byte loads when source and destination share their alignment, otherwise aligned 4-byte loads funnel-shifted into place.  Every
+// word loaded holds at least one byte of the source span, so no load leaves the span's 4-byte-aligned envelope.
+__global__ void __launch_bounds__(256) gather_kernel(const uint64_t* __restrict__ out_off, const uint64_t* __restrict__ src, uint8_t* __restrict__ out,
+                                                     uint32_t n_units) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t u = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (u >= n_units) return;
+  uint64_t n = out_off[u + 1] - out_off[u];
+  if (!n) return;
+  const uint8_t* s = reinterpret_cast<const uint8_t*>(src[u]);
+  uint8_t* d = out + out_off[u];
+  const uint64_t head = min(n, (uint64_t)((16u - ((uint32_t)(uintptr_t)d & 15u)) & 15u));
+  if (lane < head) d[lane] = s[lane];
+  d += head; s += head; n -= head;
+  const uint64_t nv = n >> 4;
+  uint4* dv = reinterpret_cast<uint4*>(d);
+  if (((uint32_t)(uintptr_t)s & 15u) == 0) {
+    const uint4* sv = reinterpret_cast<const uint4*>(s);
+    for (uint64_t k = lane; k < nv; k += 32) dv[k] = sv[k];
+  } else {
+    const uint32_t* sw = reinterpret_cast<const uint32_t*>((uintptr_t)s & ~(uintptr_t)3);
+    const uint32_t sh = ((uint32_t)(uintptr_t)s & 3u) * 8u;
+    for (uint64_t k = lane; k < nv; k += 32) {
+      const uint32_t* q = sw + 4 * k;
+      const uint32_t w0 = q[0], w1 = q[1], w2 = q[2], w3 = q[3], w4 = sh ? q[4] : 0u;
+      dv[k] = make_uint4(__funnelshift_r(w0, w1, sh), __funnelshift_r(w1, w2, sh), __funnelshift_r(w2, w3, sh), __funnelshift_r(w3, w4, sh));
+    }
+  }
+  const uint64_t t = nv << 4;
+  if (lane < n - t) d[t + lane] = s[t + lane];
+}
+
 // ---- the fused chain with host buffers (include/cfgpu.h): one H2D of the stream, every stage on the resident batch, then
-// verdicts + only the produced texts cross PCIe back
+// verdicts + only the produced texts cross PCIe back.  Legacy stream: scan, TOON, gather.  ctx->side: the substitution of the units a
+// rule matched, which needs only the scan's bitmaps and so runs beside the TOON kernel.  Host <-> device copies go through the
+// context's pinned staging.
 int cf_run_batch(cf_ctx* ctx, cf_prog* prog, cf_batch* b, const uint8_t* stream, uint64_t stream_bytes, const uint64_t* offsets, uint32_t n_units,
                  uint32_t stage_mask, const uint8_t* unit_stages, uint32_t toon_flags, int mask_max_depth, cf_verdict* verdicts, uint64_t* bitmaps_full,
                  uint8_t* out_bytes, uint64_t out_cap, uint64_t* out_offsets, uint64_t* out_needed) {
@@ -374,35 +409,52 @@ int cf_run_batch(cf_ctx* ctx, cf_prog* prog, cf_batch* b, const uint8_t* stream,
   if ((stage_mask & (CF_STAGE_SCAN | CF_STAGE_SUB)) && !prog) return CF_E_BADARG;
   if ((stage_mask & CF_STAGE_TOON) && (stage_mask & CF_STAGE_MASK)) { ctx->err = "CF_STAGE_TOON and CF_STAGE_MASK both produce the unit's output: two calls"; return CF_E_BADARG; }
   if (stage_mask & CF_STAGE_SUB) stage_mask |= CF_STAGE_SCAN;
+  if (!stream && (b->n != n_units || b->nbytes != stream_bytes)) { ctx->err = "resident run: the batch on the device is a different one"; return CF_E_BADARG; }
   struct Nvtx { Nvtx(const char* n) { nvtxRangePushA(n); } ~Nvtx() { nvtxRangePop(); } } nvtx_call("cf_run_batch");   // ranges: assemble (caller) | h2d | kernels | d2h
-  int rc = CF_OK;
+  // every return, error returns included, waits for both streams: nothing the next call's buffers are reused for stays in flight
+  struct Drain { cf_ctx* c; ~Drain() { cudaStreamSynchronize(c->side); cudaStreamSynchronize(0); } } drain{ctx};
+  const uint32_t W = prog ? prog->W : 1;
+  // pinned staging: unit_stages | bitmaps | TOON lengths + statuses | gather descriptors | substitution descriptors
+  auto r16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
+  const size_t o_bm = r16(unit_stages ? n_units : 0);
+  const size_t o_toon = o_bm + r16((stage_mask & CF_STAGE_SCAN) ? (size_t)n_units * W * 8 : 0);
+  const size_t o_gather = o_toon + r16((size_t)n_units * 8);
+  const size_t o_sub = o_gather + r16(((size_t)2 * n_units + 1) * 8);
+  int rc = cf_stage_reserve(ctx, o_sub + ((stage_mask & CF_STAGE_SUB) ? cf_sub_stage_bytes(n_units) : 0));
+  if (rc) return rc;
+  uint8_t* hs = (uint8_t*)ctx->h_stage;
   if (stream) {
     nvtxRangePushA("cf_run_batch:h2d");
     rc = cf_batch_upload(ctx, b, stream, stream_bytes, offsets, n_units, nullptr);
     nvtxRangePop();
-  } else if (b->n != n_units || b->nbytes != stream_bytes) { ctx->err = "resident run: the batch on the device is a different one"; return CF_E_BADARG; }
-  if (rc) return rc;
-  const uint32_t W = prog ? prog->W : 1;
-  std::vector<uint64_t> bm;
-  std::vector<uint32_t> tlen;
-  std::vector<int32_t> tst;
+    if (rc) return rc;
+  }
   uint8_t* d_us = nullptr;
   if (unit_stages) {
     if ((rc = cf_dev_reserve(ctx, ctx->tmp[7], n_units))) return rc;
     d_us = (uint8_t*)ctx->tmp[7].p;
-    CF_CUDA(ctx, cudaMemcpyAsync(d_us, unit_stages, n_units, cudaMemcpyHostToDevice, 0));
+    memcpy(hs, unit_stages, n_units);
+    CF_CUDA(ctx, cudaMemcpyAsync(d_us, hs, n_units, cudaMemcpyHostToDevice, 0));
   }
-  // ---- launches, back to back
+  // ---- launches, back to back; each stage's per-unit results come back in one D2H behind it
   nvtxRangePushA("cf_run_batch:kernels");
+  const uint64_t* bm = (const uint64_t*)(hs + o_bm);
+  uint32_t* tlen = (uint32_t*)(hs + o_toon);
+  const int32_t* tst = (const int32_t*)(tlen + n_units);
   if (stage_mask & CF_STAGE_SCAN) {
     if ((rc = cf_dev_reserve(ctx, ctx->tmp[6], (size_t)n_units * W * 8))) return rc;
     if ((rc = cf_scan(ctx, prog, b, (uint64_t*)ctx->tmp[6].p, nullptr))) return rc;
+    CF_CUDA(ctx, cudaMemcpyAsync(hs + o_bm, ctx->tmp[6].p, (size_t)n_units * W * 8, cudaMemcpyDeviceToHost, 0));
+    CF_CUDA(ctx, cudaEventRecord(ctx->ev_scan, 0));
   }
   if (stage_mask & CF_STAGE_TOON) {
     if ((rc = cf_dev_reserve(ctx, ctx->tmp[0], stream_bytes + 16))) return rc;
-    if ((rc = cf_dev_reserve(ctx, ctx->tmp[1], (size_t)n_units * 4))) return rc;
-    if ((rc = cf_dev_reserve(ctx, ctx->tmp[2], (size_t)n_units * 4))) return rc;
-    if ((rc = toon_launch(ctx, b, toon_flags & ~(CF_TOON_PARSE_ONLY | CF_TOON_SEQUENTIAL | CF_RUN_OUTPUTS_RESIDENT), (uint8_t*)ctx->tmp[0].p, (uint32_t*)ctx->tmp[1].p, (int32_t*)ctx->tmp[2].p, d_us, 0))) return rc;
+    if ((rc = cf_dev_reserve(ctx, ctx->tmp[1], (size_t)n_units * 8))) return rc;     // lengths | statuses
+    uint32_t* d_len = (uint32_t*)ctx->tmp[1].p;
+    if ((rc = toon_launch(ctx, b, toon_flags & ~(CF_TOON_PARSE_ONLY | CF_TOON_SEQUENTIAL | CF_RUN_OUTPUTS_RESIDENT), (uint8_t*)ctx->tmp[0].p, d_len,
+                          (int32_t*)(d_len + n_units), d_us, 0))) return rc;
+    CF_CUDA(ctx, cudaMemcpyAsync(tlen, d_len, (size_t)n_units * 8, cudaMemcpyDeviceToHost, 0));
+    CF_CUDA(ctx, cudaEventRecord(ctx->ev_toon, 0));
   }
   nvtxRangePop();
   // ---- results of the launches
@@ -410,9 +462,8 @@ int cf_run_batch(cf_ctx* ctx, cf_prog* prog, cf_batch* b, const uint8_t* stream,
   for (uint32_t i = 0; i < n_units; ++i) { verdicts[i].match_bitmap = 0; verdicts[i].flags = 0; verdicts[i].out_len = 0; verdicts[i].aux = 0; verdicts[i].reserved = 0; }
   std::vector<uint32_t> dirty;
   if (stage_mask & CF_STAGE_SCAN) {
-    bm.resize((size_t)n_units * W);
-    CF_CUDA(ctx, cudaMemcpy(bm.data(), ctx->tmp[6].p, bm.size() * 8, cudaMemcpyDeviceToHost));
-    if (bitmaps_full) memcpy(bitmaps_full, bm.data(), bm.size() * 8);
+    CF_CUDA(ctx, cudaEventSynchronize(ctx->ev_scan));
+    if (bitmaps_full) memcpy(bitmaps_full, bm, (size_t)n_units * W * 8);
     std::vector<uint64_t> rule_mask(W, 0);
     for (int pi : prog->ordered_pat) rule_mask[(size_t)pi / 64] |= 1ull << (pi % 64);
     for (uint32_t i = 0; i < n_units; ++i) {
@@ -424,36 +475,28 @@ int cf_run_batch(cf_ctx* ctx, cf_prog* prog, cf_batch* b, const uint8_t* stream,
       }
     }
   }
-  if (stage_mask & CF_STAGE_TOON) {
-    tlen.resize(n_units); tst.resize(n_units);
-    CF_CUDA(ctx, cudaMemcpy(tlen.data(), ctx->tmp[1].p, (size_t)n_units * 4, cudaMemcpyDeviceToHost));
-    CF_CUDA(ctx, cudaMemcpy(tst.data(), ctx->tmp[2].p, (size_t)n_units * 4, cudaMemcpyDeviceToHost));
-  }
-  // ---- regex_filter rewriting of the (few) units a rule matched
-  std::vector<uint8_t> sub_bytes;
-  std::vector<uint64_t> sub_off;
+  // ---- regex_filter rewriting of the (few) units a rule matched, on the side stream while the TOON kernel runs
+  const uint64_t* rec = nullptr;
   if (!dirty.empty()) {
-    sub_off.assign(dirty.size() + 1, 0);
-    uint64_t need = 0;
-    sub_bytes.resize(1 << 16);
-    rc = cf_sub_host(ctx, prog, b, dirty.data(), (uint32_t)dirty.size(), sub_bytes.data(), sub_bytes.size(), sub_off.data(), &need);
-    if (rc == CF_E_CAPACITY && need > sub_bytes.size()) {
-      sub_bytes.resize(need);
-      rc = cf_sub_host(ctx, prog, b, dirty.data(), (uint32_t)dirty.size(), sub_bytes.data(), sub_bytes.size(), sub_off.data(), &need);
-    }
-    if (rc) return rc;
+    CF_CUDA(ctx, cudaStreamWaitEvent(ctx->side, ctx->ev_scan, 0));
+    if ((rc = cf_sub_device(ctx, prog, b, offsets, dirty.data(), (uint32_t)dirty.size(), ctx->side, hs + o_sub, &rec))) return rc;
+    CF_CUDA(ctx, cudaEventRecord(ctx->ev_sub, ctx->side));
+    CF_CUDA(ctx, cudaStreamWaitEvent(0, ctx->ev_sub, 0));
     for (size_t k = 0; k < dirty.size(); ++k) {
       const uint32_t i = dirty[k];
       verdicts[i].flags |= CF_V_REWRITTEN;
-      verdicts[i].out_len = (uint32_t)(sub_off[k + 1] - sub_off[k]);
-      if ((stage_mask & CF_STAGE_TOON) && (!unit_stages || (unit_stages[i] & CF_STAGE_TOON))) { verdicts[i].flags |= CF_V_RESUBMIT; tst[i] = CF_TOON_SKIPPED; tlen[i] = 0; }
+      verdicts[i].out_len = (uint32_t)rec[2 * k + 1];
+      if ((stage_mask & CF_STAGE_TOON) && (!unit_stages || (unit_stages[i] & CF_STAGE_TOON))) verdicts[i].flags |= CF_V_RESUBMIT;
     }
   }
-  if (stage_mask & CF_STAGE_TOON)
+  if (stage_mask & CF_STAGE_TOON) {
+    CF_CUDA(ctx, cudaEventSynchronize(ctx->ev_toon));
     for (uint32_t i = 0; i < n_units; ++i) {
-      verdicts[i].aux = tst[i];
-      if (tst[i] == CF_TOON_CONVERTED && !(verdicts[i].flags & CF_V_REWRITTEN)) { verdicts[i].flags |= CF_V_TOON; verdicts[i].out_len = tlen[i]; }
+      const int32_t s = (verdicts[i].flags & CF_V_RESUBMIT) ? CF_TOON_SKIPPED : tst[i];   // the caller encodes the rewritten text
+      verdicts[i].aux = s;
+      if (s == CF_TOON_CONVERTED && !(verdicts[i].flags & CF_V_REWRITTEN)) { verdicts[i].flags |= CF_V_TOON; verdicts[i].out_len = tlen[i]; }
     }
+  }
   // ---- masking on the same upload (sequential kernel; its own gather)
   if (stage_mask & CF_STAGE_MASK) {
     std::vector<int32_t> mst(n_units);
@@ -470,7 +513,8 @@ int cf_run_batch(cf_ctx* ctx, cf_prog* prog, cf_batch* b, const uint8_t* stream,
     out_offsets[n_units] = moff[n_units];
     return CF_OK;
   }
-  // ---- pack the outputs: TOON texts gathered on the device (one D2H), rewritten texts from the substitution call
+  // ---- pack the outputs: TOON texts (input layout in tmp[0]) and rewritten texts (substitution scratch, or the unit itself) in one
+  // gather at their final offsets, then one D2H straight into out_bytes unless they stay resident
   uint64_t total = 0;
   for (uint32_t i = 0; i < n_units; ++i) { out_offsets[i] = total; total += verdicts[i].out_len; }
   out_offsets[n_units] = total;
@@ -478,32 +522,23 @@ int cf_run_batch(cf_ctx* ctx, cf_prog* prog, cf_batch* b, const uint8_t* stream,
   const bool keep = (toon_flags & CF_RUN_OUTPUTS_RESIDENT) != 0;
   ctx->run_out = nullptr; ctx->run_out_bytes = 0;
   if (!keep && (total > out_cap || (!out_bytes && total))) { ctx->err = "output buffer too small"; return CF_E_CAPACITY; }
-  if (keep && total && (rc = cf_dev_reserve(ctx, ctx->tmp[4], total))) return rc;
-  if ((stage_mask & CF_STAGE_TOON) && total) {
-    // gather the TOON texts on the device AT THEIR FINAL OFFSETS (rewritten units leave holes), then ONE D2H straight into out_bytes
-    std::vector<uint32_t> glen(n_units);
-    bool any = false;
-    for (uint32_t i = 0; i < n_units; ++i) { glen[i] = (verdicts[i].flags & CF_V_TOON) ? verdicts[i].out_len : 0u; any = any || glen[i]; }
-    if (any) {
-      if ((rc = cf_dev_reserve(ctx, ctx->tmp[3], ((size_t)n_units + 1) * 8))) return rc;
-      if ((rc = cf_dev_reserve(ctx, ctx->tmp[4], total))) return rc;
-      CF_CUDA(ctx, cudaMemcpyAsync(ctx->tmp[3].p, out_offsets, ((size_t)n_units + 1) * 8, cudaMemcpyHostToDevice, 0));
-      CF_CUDA(ctx, cudaMemcpyAsync(ctx->tmp[1].p, glen.data(), (size_t)n_units * 4, cudaMemcpyHostToDevice, 0));
-      compact_kernel<<<n_units, 128>>>((const uint8_t*)ctx->tmp[0].p, 1, 0, b->d_offsets, (const uint32_t*)ctx->tmp[1].p, (const uint64_t*)ctx->tmp[3].p, (uint8_t*)ctx->tmp[4].p, n_units);
-      ctx->launches++;
-      CF_CUDA(ctx, cudaGetLastError());
-      if (!keep) CF_CUDA(ctx, cudaMemcpy(out_bytes, ctx->tmp[4].p, total, cudaMemcpyDeviceToHost));
-    }
-  }
-  for (size_t k = 0; k < dirty.size(); ++k) {
-    const uint32_t i = dirty[k];
-    if (!verdicts[i].out_len) continue;
-    // resident outputs: the rewritten text is still in the substitution call's device buffer (ctx->tmp[14], packed at sub_off)
-    if (keep) CF_CUDA(ctx, cudaMemcpyAsync((uint8_t*)ctx->tmp[4].p + out_offsets[i], (const uint8_t*)ctx->tmp[14].p + sub_off[k], verdicts[i].out_len, cudaMemcpyDeviceToDevice, 0));
-    else memcpy(out_bytes + out_offsets[i], sub_bytes.data() + sub_off[k], verdicts[i].out_len);
+  if (total) {
+    uint64_t* h_src = (uint64_t*)(hs + o_gather);          // src[n] | out_off[n + 1]: one H2D
+    const uintptr_t toon_out = (uintptr_t)ctx->tmp[0].p, d_stream = (uintptr_t)(b->d_buf + cf::FRONT_PAD), scratch = (uintptr_t)ctx->tmp[8].p;
+    for (uint32_t i = 0; i < n_units; ++i) h_src[i] = (verdicts[i].flags & CF_V_TOON) ? toon_out + offsets[i] : 0;
+    for (size_t k = 0; k < dirty.size(); ++k) h_src[dirty[k]] = rec[2 * k] == ~0ull ? d_stream + offsets[dirty[k]] : scratch + rec[2 * k];
+    memcpy(h_src + n_units, out_offsets, ((size_t)n_units + 1) * 8);
+    if ((rc = cf_dev_reserve(ctx, ctx->tmp[3], ((size_t)2 * n_units + 1) * 8))) return rc;
+    if ((rc = cf_dev_reserve(ctx, ctx->tmp[4], total))) return rc;
+    const uint64_t* d_src = (const uint64_t*)ctx->tmp[3].p;
+    CF_CUDA(ctx, cudaMemcpyAsync(ctx->tmp[3].p, h_src, ((size_t)2 * n_units + 1) * 8, cudaMemcpyHostToDevice, 0));
+    gather_kernel<<<(n_units + 7) / 8, 256, 0, 0>>>(d_src + n_units, d_src, (uint8_t*)ctx->tmp[4].p, n_units);
+    ctx->launches++;
+    CF_CUDA(ctx, cudaGetLastError());
+    if (!keep) CF_CUDA(ctx, cudaMemcpyAsync(out_bytes, ctx->tmp[4].p, total, cudaMemcpyDeviceToHost, 0));
+    CF_CUDA(ctx, cudaStreamSynchronize(0));
   }
   if (keep) {
-    CF_CUDA(ctx, cudaStreamSynchronize(0));
     ctx->run_out = total ? (const uint8_t*)ctx->tmp[4].p : nullptr;
     ctx->run_out_bytes = total;
   }
