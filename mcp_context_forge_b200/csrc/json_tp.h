@@ -67,7 +67,7 @@ static const uint32_t RING = 256, MAXD = 64, KH_CAP = 256;
 static const uint32_t TOK_WIN = 192;      // tokens of one 1 KiB step pushed through the ring at a time (a window never overtakes the 32-token batches)
 static const uint32_t UNSET = 0xFFFFFFFFu;
 struct Shared {
-  uint32_t ring_pos[RING], ring_len[RING], ring_meta[RING];
+  uint32_t ring_pos[RING], ring_len[RING], ring_meta[RING];   // tokenize | analyze: ring_pos[j], ring_len[j] = the key whose hash is kh[j]
   // analyze: container stack            | emit: frame stack (same storage)
   uint32_t open_idx[MAXD];             // token index of the opener      | frame mode
   uint32_t cnt[MAXD];                  // children (values) so far       | children so far
@@ -91,6 +91,10 @@ enum : uint32_t {
   C_CRASH = 256,         // ... and arrived before any key-set mismatch: _try_columnar_encoding raises AttributeError
   C_PERMUTED = 512,      // some row lists the first row's keys in another order (columnar output needs a gather)
   C_ROW0_SIMPLE = 1024,  // the first row's values are primitives: its j-th key is token row0 + 1 + 2j
+  C_ITEM_HEAD = 2048,    // the first member of an object that is an element of an array: as a list item's first value, toon.py:400-404
+                         // tries the array as columnar without a type check, so only here does AF_CRASH / AF_MIXED matter
+  C_R0KEYS = 8192,       // (resolve_mixed) the first row is not simple; its keys stay at kh / ring_pos / ring_len[khbase - row0_n ..)
+                         // (the later rows' keys are hashed from khbase on) so that every later row's key set is compared with it
   // objects
   C_ALIGNED = 16,        // keys equal the first row's, position by position
   C_VALS_SIMPLE = 32,    // all member values are primitives
@@ -362,7 +366,7 @@ TP_FN uint32_t nondict_element(uint32_t afl, uint32_t row0, uint32_t row0_n) {
   afl &= ~C_ALL_OBJ;
   if (row0 && !(afl & C_ND_SEEN)) {
     afl |= C_ND_SEEN;
-    if ((afl & C_KEYSET_OK) && (afl & C_ROW0_SIMPLE) && row0_n != 0 && row0_n != UNSET) afl |= C_CRASH;
+    if ((afl & C_KEYSET_OK) && (afl & (C_ROW0_SIMPLE | C_R0KEYS)) && row0_n != 0 && row0_n != UNSET) afl |= C_CRASH;
   }
   return afl;
 }
@@ -784,6 +788,7 @@ TP_FN bool table_candidate(const Shared& sh, uint32_t top) {
 // Generic mode: tokens [i, i+m) with one walk over their brackets.  Returns the number of tokens consumed: the walk stops in
 // front of a row opener `{` of a table candidate (unless it is the batch's first token and `force`), so that table mode can
 // take over.
+template <bool RESOLVE_MIXED>
 TP_FN uint32_t an_batch(const uint8_t* s, GTok* toks, uint32_t tok_cap, Shared& sh, AnState& st, uint32_t i, uint32_t m, bool force) {
   const uint32_t l = tpw::lane();
   const uint32_t ltm = tpw::lt_mask();
@@ -833,7 +838,7 @@ TP_FN uint32_t an_batch(const uint8_t* s, GTok* toks, uint32_t tok_cap, Shared& 
           // duplicate-key screen on the hashes (a repeated hash, real duplicate or not, goes to the sequential encoder)
           const uint32_t kb = T_khb;
           const bool mine = inrun && kind == K_KEY;
-          if (mine) { if (kb + ord >= KH_CAP) fb = FB_KH_CAP; else sh.kh[kb + ord] = hash; }
+          if (mine) { if (kb + ord >= KH_CAP) fb = FB_KH_CAP; else { sh.kh[kb + ord] = hash; if (RESOLVE_MIXED) { sh.ring_pos[kb + ord] = pos; sh.ring_len[kb + ord] = len; } } }
           tpw::sync();
           if (mine && kb + ord < KH_CAP) for (uint32_t j = kb; j < kb + ord; ++j) if (sh.kh[j] == hash) { fb = FB_DUP_HASH; break; }
           // table detection: the keys of every later row against the first row's, position by position
@@ -851,6 +856,23 @@ TP_FN uint32_t an_batch(const uint8_t* s, GTok* toks, uint32_t tok_cap, Shared& 
               }
               const bool anym = tpw::any(mism), anyd = tpw::any(diff);
               if (anym) T_cfl = (T_cfl & ~C_ALIGNED) | (anyd ? C_DIFFSET : 0u);
+            } else if (RESOLVE_MIXED && (pfl & C_R0KEYS) && (pfl & C_KEYSET_OK) && !(pfl & C_ND_SEEN)) {
+              // a later row of an array whose first row is not simple: is each key one of the first row's?
+              const uint32_t rn = sh.row0_n[par], r0k = sh.khbase[par] - rn;
+              bool diff = false;
+              if (mine) {
+                const auto same = [&](uint32_t j) {            // hash and length screen in shared memory, then the bytes
+                  if (sh.kh[r0k + j] != hash || sh.ring_len[r0k + j] != len) return false;
+                  const uint8_t* a = s + sh.ring_pos[r0k + j];
+                  for (uint32_t q = 0; q < len; ++q) if (a[q] != s[pos + q]) return false;
+                  return true;
+                };
+                if (ord >= rn || !same(ord)) {
+                  diff = true;
+                  for (uint32_t j = 0; j < rn; ++j) if (same(j)) { diff = false; break; }
+                }
+              }
+              if (tpw::any(diff)) T_cfl |= C_DIFFSET;
             }
           }
           tpw::sync();
@@ -864,6 +886,7 @@ TP_FN uint32_t an_batch(const uint8_t* s, GTok* toks, uint32_t tok_cap, Shared& 
     const uint32_t eidx = i + e;
     if (ek <= K_OPEN_ARR) {
       uint32_t newkb = 0;
+      bool item_head = false;
       if (sp == 0) { if (ecomma || ecolon || root_cnt) ubad = true; ++root_cnt; }
       else {
         const uint32_t ord = T_cnt;
@@ -878,11 +901,12 @@ TP_FN uint32_t an_batch(const uint8_t* s, GTok* toks, uint32_t tok_cap, Shared& 
         newkb = T_khb + (isobj ? ord + 1 : 0u);
         T_cnt = ord + 1;
         if (!isobj && ord == 0 && ek == K_OPEN_OBJ) T_r0i = eidx + 1;
+        if (RESOLVE_MIXED) item_head = ek == K_OPEN_ARR && isobj && ord == 0 && sp >= 2 && !(sh.cfl[sp - 2] & C_OBJ);
       }
       if (sp >= MAXD) { uunsup = true; break; }
       if (sp && l == 0) { const uint32_t k = sp - 1; sh.open_idx[k] = T_oi; sh.cnt[k] = T_cnt; sh.cfl[k] = T_cfl; sh.khbase[k] = T_khb; sh.row0_idx[k] = T_r0i; sh.row0_n[k] = T_r0n; sh.open_w[k] = T_ow; }
       T_oi = eidx; T_cnt = 0; T_khb = newkb < KH_CAP ? newkb : KH_CAP;
-      T_cfl = ek == K_OPEN_OBJ ? (C_OBJ | C_ALIGNED | C_VALS_SIMPLE) : (C_ALL_SIMPLE | C_ALL_OBJ | C_KEYSET_OK | C_ROWS_SIMPLE);
+      T_cfl = ek == K_OPEN_OBJ ? (C_OBJ | C_ALIGNED | C_VALS_SIMPLE) : (C_ALL_SIMPLE | C_ALL_OBJ | C_KEYSET_OK | C_ROWS_SIMPLE | (item_head ? C_ITEM_HEAD : 0u));
       T_r0i = 0; T_r0n = UNSET; T_ow = gt_make(ek, 0, ecomma, ecolon, 0);
       ++sp;
       tpw::sync();
@@ -899,7 +923,10 @@ TP_FN uint32_t an_batch(const uint8_t* s, GTok* toks, uint32_t tok_cap, Shared& 
         const uint32_t mode = nn == 0 ? AM_EMPTY : col ? AM_COLUMNAR : (tfl & C_ALL_SIMPLE) ? AM_INLINE : AM_ITEMS;
         if (col && (tfl & C_PERMUTED)) ufb = FB_ROW_ORDER;          // the rows need a gather: sequential encoder
         uint32_t xf = 0;
-        if (T_r0i && !(tfl & C_ALL_OBJ)) xf = (tfl & C_CRASH) ? AF_CRASH : (!(tfl & C_ROW0_SIMPLE) && T_r0n != 0) ? AF_MIXED : 0u;
+        // the second pass leaves the verdict open only for a first row whose keys were not kept (too many open keys), unless a row
+        // count already differed
+        if (T_r0i && !(tfl & C_ALL_OBJ))
+          xf = (tfl & C_CRASH) ? AF_CRASH : (!(tfl & (C_ROW0_SIMPLE | C_R0KEYS)) && (!RESOLVE_MIXED || (tfl & C_KEYSET_OK)) && T_r0n != 0) ? AF_MIXED : 0u;
         pk = K_OPEN_ARR; pf = mode | xf;
       }
       if (l == 0 && oi < tok_cap) toks[oi].w = gt_patch(T_ow, pk, pf, nn & GT_MAXLEN);
@@ -912,6 +939,7 @@ TP_FN uint32_t an_batch(const uint8_t* s, GTok* toks, uint32_t tok_cap, Shared& 
           if (!(tfl & C_VALS_SIMPLE)) T_cfl &= ~C_ROWS_SIMPLE;
           if (oi + 1 == T_r0i) {                                     // the first row
             if (tfl & C_VALS_SIMPLE) T_cfl |= C_ROW0_SIMPLE;
+            else if (RESOLVE_MIXED && (T_cfl & C_ITEM_HEAD) && nn != 0 && T_khb + 2 * nn <= KH_CAP) { T_cfl |= C_R0KEYS; T_khb += nn; }   // keep its keys
             T_r0n = nn;
           } else if (T_r0n != UNSET && (T_cfl & C_KEYSET_OK) && !(T_cfl & C_ND_SEEN)) {
             // same key set?  (no duplicate keys here — those went to the sequential encoder — so equal counts + every key found = equal sets)
@@ -989,6 +1017,7 @@ TP_FN uint32_t an_rows(const uint8_t* s, GTok* toks, uint32_t ntok, Shared& sh, 
   return ngood;
 }
 
+template <bool RESOLVE_MIXED>
 TP_FN int analyze(const uint8_t* s, GTok* toks, uint32_t ntok, uint32_t tok_cap, Shared& sh, uint8_t* stage) {
   AnState st; st.sp = 0; st.root_cnt = 0; st.last_was_key = 0; st.status = 0;
   uint32_t i = 0;
@@ -1002,7 +1031,7 @@ TP_FN int analyze(const uint8_t* s, GTok* toks, uint32_t ntok, uint32_t tok_cap,
       continue;
     }
     const uint32_t m = ntok - i > 32 ? 32u : ntok - i;
-    const uint32_t c = an_batch(s, toks, tok_cap, sh, st, i, m, force);
+    const uint32_t c = an_batch<RESOLVE_MIXED>(s, toks, tok_cap, sh, st, i, m, force);
     force = false;
     i += c;
   }
@@ -1325,16 +1354,25 @@ TP_FN int emit(const uint8_t* s, const GTok* toks, uint32_t ntok, uint8_t* out, 
 // conversion is only kept when strictly smaller).  Returns a TS_* status, TS_FALLBACK (| reason << 8) when the sequential
 // encoder has to redo the unit.
 // `stage` = STAGE bytes of per-warp scratch, 16-byte aligned (shared memory on the GPU).
-TP_FN int toon_unit(const uint8_t* s, uint32_t n, GTok* toks, uint32_t tok_cap, uint8_t* out, uint32_t out_cap, uint32_t* out_len, Shared& sh,
-                    uint8_t* stage, bool report_errors) {
+// RESOLVE_MIXED: decide mixed list-item arrays whose first row is not simple (C_R0KEYS) instead of returning FB_MIXED_ITEM.  Its key
+// bookkeeping would slow every nested unit down, so the first pass over a batch is compiled without it and a second pass with it runs
+// over the units that came back with FB_MIXED_ITEM only.
+template <bool RESOLVE_MIXED>
+TP_FN int toon_unit_t(const uint8_t* s, uint32_t n, GTok* toks, uint32_t tok_cap, uint8_t* out, uint32_t out_cap, uint32_t* out_len, Shared& sh,
+                      uint8_t* stage, bool report_errors) {
   uint32_t ntok = 0;
   int st = tokenize(s, n, toks, tok_cap, sh, stage, &ntok);
   if (st) return st;
   tpw::sync();
-  st = analyze(s, toks, ntok, tok_cap, sh, stage);
+  st = analyze<RESOLVE_MIXED>(s, toks, ntok, tok_cap, sh, stage);
   if (st) return st;
   tpw::sync();
   return emit(s, toks, ntok, out, out_cap, out_len, sh, stage, report_errors);
+}
+TP_FN int toon_unit(const uint8_t* s, uint32_t n, GTok* toks, uint32_t tok_cap, uint8_t* out, uint32_t out_cap, uint32_t* out_len, Shared& sh,
+                    uint8_t* stage, bool report_errors, bool resolve_mixed = false) {
+  return resolve_mixed ? toon_unit_t<true>(s, n, toks, tok_cap, out, out_cap, out_len, sh, stage, report_errors)
+                       : toon_unit_t<false>(s, n, toks, tok_cap, out, out_cap, out_len, sh, stage, report_errors);
 }
 
 }  // namespace cftp
