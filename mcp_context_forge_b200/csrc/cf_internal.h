@@ -34,6 +34,8 @@ struct cf_ctx {
   struct DevBuf { void* p = nullptr; size_t cap = 0; };
   DevBuf tmp[16];                   // grow-only device scratch of the *_host entry points (no cudaMalloc per call)
   DevBuf d_tok, d_ntok;             // structural index of the current batch (json_index_kernel)
+  DevBuf toon_order;                // TOON first pass: units in cost order (uint32 per unit)
+  DevBuf toon_sort;                 // ... and the sort behind it: unit indices | keys in | keys out | radix-sort temp storage
   void* h_stage = nullptr;          // pinned host staging for gathered results
   size_t h_stage_bytes = 0;
   const uint8_t* run_out = nullptr;   // device buffer of the last CF_RUN_OUTPUTS_RESIDENT call

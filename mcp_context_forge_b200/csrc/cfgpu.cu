@@ -976,6 +976,7 @@ void cf_shutdown(cf_ctx* ctx) {
   cudaFree(ctx->d_toon_scratch);
   for (auto& t : ctx->tmp) cudaFree(t.p);
   cudaFree(ctx->d_tok.p); cudaFree(ctx->d_ntok.p);
+  cudaFree(ctx->toon_order.p); cudaFree(ctx->toon_sort.p);
   if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
   if (ctx->side) cudaStreamDestroy(ctx->side);
   for (cudaEvent_t e : {ctx->ev_scan, ctx->ev_toon, ctx->ev_sub}) if (e) cudaEventDestroy(e);

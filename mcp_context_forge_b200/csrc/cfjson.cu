@@ -5,6 +5,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <cub/device/device_radix_sort.cuh>
 #include <nvtx3/nvToolsExt.h>
 
 #include "cf_internal.h"
@@ -100,6 +101,10 @@ __global__ void __launch_bounds__(128) json_index_kernel(const uint8_t* __restri
 // over as mixed list-item arrays (FB_MIXED_ITEM) first get a second token-parallel pass that decides them (RESOLVE_PASS): it
 // costs key comparisons the first pass saves on every other unit, and a warp is far quicker than the sequential encoder's one
 // thread per unit.
+// The first pass takes its units in cost order (toon_order_kernel + a stable radix sort, heaviest first): a CTA holds its slot
+// until its slowest warp is done, and a nested unit costs about three tabular ones, so CTAs that mix shapes idle most of their
+// warps.  In cost order each CTA, and at any moment each SM, runs units of one kind.  The resolving pass and the sequential
+// encoder keep the natural order: their few units are then spread over many SMs instead of packed into a few CTAs.
 // ------------------------------------------------------------------------------------------------
 static const uint32_t TP_WARPS = 8;
 static const uint32_t TP_TOK_SLACK = 64;               // token capacity of unit u: len/2 + TP_TOK_SLACK
@@ -108,11 +113,13 @@ static const uint32_t TP_SMEM = TP_WARPS * TP_WARP_SMEM;                        
 template <bool RESOLVE_PASS>
 __global__ void __launch_bounds__(TP_WARPS * 32, 2) toon_tp_kernel(const uint8_t* __restrict__ stream, const uint64_t* __restrict__ offsets, uint32_t n_units,
                                                                     cftp::GTok* __restrict__ toks, uint8_t* __restrict__ out, uint32_t* __restrict__ out_len,
-                                                                    int32_t* __restrict__ status, uint32_t flags, const uint8_t* __restrict__ unit_stages) {
+                                                                    int32_t* __restrict__ status, uint32_t flags, const uint8_t* __restrict__ unit_stages,
+                                                                    const uint32_t* __restrict__ order) {
   extern __shared__ __align__(16) uint8_t tp_smem[];
   const uint32_t lane = threadIdx.x & 31, wic = threadIdx.x >> 5;
-  const uint32_t u = blockIdx.x * TP_WARPS + wic;
-  if (u >= n_units) return;
+  const uint32_t slot = blockIdx.x * TP_WARPS + wic;
+  if (slot >= n_units) return;
+  const uint32_t u = RESOLVE_PASS ? slot : order[slot];
   if (RESOLVE_PASS) { if (status[u] != cftp::TS_FALLBACK || out_len[u] != cftp::FB_MIXED_ITEM) return; }
   else if (unit_stages && !(unit_stages[u] & CF_STAGE_TOON)) { if (lane == 0) { status[u] = CF_TOON_SKIPPED; out_len[u] = 0; } return; }
   cftp::Shared& sh = *reinterpret_cast<cftp::Shared*>(tp_smem + (size_t)wic * TP_WARP_SMEM);
@@ -133,6 +140,52 @@ __global__ void __launch_bounds__(TP_WARPS * 32, 2) toon_tp_kernel(const uint8_t
   if (lane == 0) {
     status[u] = st & 0xFF;
     out_len[u] = (st & 0xFF) == cfj::TS_CONVERTED ? ol : (uint32_t)st >> 8;
+  }
+}
+
+// cost key of each unit for the first pass's order (json_tp.h order_events over the unit's first ORDER_WINDOW bytes, clamped to
+// 8 bits; 0 for units that do not take TOON, empty and oversized ones), one warp per unit with 16-byte loads; idx[u] = u.
+// The loads are rounded out to the 16-byte grid: the batch buffer's front and tail padding keep them inside it, and the bytes
+// outside the window are zeroed.
+__global__ void __launch_bounds__(256) toon_order_kernel(const uint8_t* __restrict__ stream, const uint64_t* __restrict__ offsets, uint32_t n_units,
+                                                         const uint8_t* __restrict__ unit_stages, uint8_t* __restrict__ key, uint32_t* __restrict__ idx) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t u = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (u >= n_units) return;
+  const uint64_t b = offsets[u];
+  const uint64_t len = offsets[u + 1] - b - 1;
+  uint32_t ev = 0;
+  if (len && len <= 0x7FFFFFFFull && !(unit_stages && !(unit_stages[u] & CF_STAGE_TOON))) {
+    const uint32_t win = len < cftp::ORDER_WINDOW ? (uint32_t)len : cftp::ORDER_WINDOW;
+    const uint32_t lead = (uint32_t)((uintptr_t)(stream + b) & 15u);
+    const uint4* g = reinterpret_cast<const uint4*>(stream + b - lead);
+    const uint32_t nchunks = (lead + win + 15) >> 4;
+    uint32_t carry = 0;                                    // the last word of the previous round's lane 31
+    for (uint32_t c0 = 0; c0 < nchunks; c0 += 32) {
+      const uint32_t c = c0 + lane;
+      uint32_t w[4] = {0, 0, 0, 0};
+      if (c < nchunks) {
+        const uint4 v = g[c];
+        w[0] = v.x; w[1] = v.y; w[2] = v.z; w[3] = v.w;
+        const int32_t p0 = (int32_t)(16 * c) - (int32_t)lead;   // unit position of the chunk's byte 0
+        if (p0 < 0 || p0 + 16 > (int32_t)win) {
+#pragma unroll
+          for (uint32_t k = 0; k < 16; ++k) {
+            const int32_t p = p0 + (int32_t)k;
+            if (p < 0 || p >= (int32_t)win) w[k >> 2] &= ~(0xFFu << (8 * (k & 3)));
+          }
+        }
+      }
+      uint32_t prev = __shfl_up_sync(0xFFFFFFFFu, w[3], 1);
+      if (lane == 0) prev = carry;
+      carry = __shfl_sync(0xFFFFFFFFu, w[3], 31);
+      ev += cftp::order_events(prev, w[0]) + cftp::order_events(w[0], w[1]) + cftp::order_events(w[1], w[2]) + cftp::order_events(w[2], w[3]);
+    }
+    ev = __reduce_add_sync(0xFFFFFFFFu, ev);
+  }
+  if (lane == 0) {
+    key[u] = (uint8_t)(ev < 255u ? ev : 255u);
+    idx[u] = u;
   }
 }
 
@@ -214,23 +267,41 @@ static int toon_launch(cf_ctx* ctx, cf_batch* b, uint32_t flags, uint8_t* d_out,
     CF_CUDA(ctx, cudaMalloc(&ctx->d_toon_scratch, need + need / 4));
     ctx->toon_scratch_bytes = need + need / 4;
   }
+  const bool tp = !(flags & (CF_TOON_PARSE_ONLY | CF_TOON_SEQUENTIAL));
+  // the first pass's unit order: key + stable radix sort over its 8 bits, descending; toon_sort = indices | keys in | keys out | temp
+  const size_t o_kin = (size_t)b->n * 4, o_kout = o_kin + b->n, o_tmp = (o_kout + b->n + 255) & ~(size_t)255;
+  size_t sort_tmp = 0;
+  if (tp) {
+    CF_CUDA(ctx, cub::DeviceRadixSort::SortPairsDescending(nullptr, sort_tmp, (const uint8_t*)nullptr, (uint8_t*)nullptr, (const uint32_t*)nullptr,
+                                                           (uint32_t*)nullptr, (int)b->n, 0, 8, st));
+    int rc;
+    if ((rc = cf_dev_reserve(ctx, ctx->toon_order, (size_t)b->n * 4))) return rc;
+    if ((rc = cf_dev_reserve(ctx, ctx->toon_sort, o_tmp + sort_tmp))) return rc;
+  }
   const bool prof = ctx->prof_on && (size_t)ctx->prof_used + 2 <= ctx->prof_ev.size();
   if (prof) cudaEventRecord(ctx->prof_ev[ctx->prof_used], st);
-  if (!(flags & (CF_TOON_PARSE_ONLY | CF_TOON_SEQUENTIAL))) {
+  if (tp) {
     static bool smem_set = false;
     if (!smem_set) {
       CF_CUDA(ctx, cudaFuncSetAttribute(toon_tp_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TP_SMEM));
       CF_CUDA(ctx, cudaFuncSetAttribute(toon_tp_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TP_SMEM));
       smem_set = true;
     }
+    uint8_t* srt = (uint8_t*)ctx->toon_sort.p;
+    uint32_t* order = (uint32_t*)ctx->toon_order.p;
+    toon_order_kernel<<<(b->n + 7) / 8, 256, 0, st>>>(b->d_buf + cf::FRONT_PAD, b->d_offsets, b->n, d_unit_stages, srt + o_kin, (uint32_t*)srt);
+    ctx->launches++;
+    CF_CUDA(ctx, cudaGetLastError());
+    CF_CUDA(ctx, cub::DeviceRadixSort::SortPairsDescending(srt + o_tmp, sort_tmp, srt + o_kin, srt + o_kout, (const uint32_t*)srt, order, (int)b->n, 0, 8, st));
+    ctx->launches++;
     const uint32_t grid = (b->n + TP_WARPS - 1) / TP_WARPS;
     toon_tp_kernel<false><<<grid, TP_WARPS * 32, TP_SMEM, st>>>(b->d_buf + cf::FRONT_PAD, b->d_offsets, b->n, (cftp::GTok*)ctx->d_toon_scratch, d_out, d_out_len,
-                                                                d_status, flags, d_unit_stages);
+                                                                d_status, flags, d_unit_stages, order);
     ctx->launches++;
     CF_CUDA(ctx, cudaGetLastError());
     if (!(flags & CF_TOON_NO_HANDOVER)) {
       toon_tp_kernel<true><<<grid, TP_WARPS * 32, TP_SMEM, st>>>(b->d_buf + cf::FRONT_PAD, b->d_offsets, b->n, (cftp::GTok*)ctx->d_toon_scratch, d_out, d_out_len,
-                                                                 d_status, flags, d_unit_stages);
+                                                                 d_status, flags, d_unit_stages, nullptr);
       ctx->launches++;
       CF_CUDA(ctx, cudaGetLastError());
     }

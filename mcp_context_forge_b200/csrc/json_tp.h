@@ -187,6 +187,19 @@ TP_FN uint32_t swar_eq(uint32_t w, uint32_t c) { const uint32_t x = w ^ (c * 0x0
 TP_FN uint32_t swar_range7(uint32_t x7, uint32_t lo, uint32_t hi) { return (x7 + (0x80u - lo) * 0x01010101u) & ~(x7 + (0x7Fu - hi) * 0x01010101u) & 0x80808080u; }
 TP_FN uint32_t gather4(uint32_t f) { return (((f >> 7) * 0x00204081u) >> 21) & 15u; }   // flags at bits 7,15,23,31 -> nibble
 
+// ---- cost key of a unit (toon_order_kernel, cfjson.cu): the first pass runs units heaviest first ----
+// Estimate of the events the generic bracket walk handles in the 4 bytes of w (prev = the 4 bytes before them, 0 before the
+// unit): every '{' and '[', except a '{' right after "}," or "}, " -- the next row of an array of objects, which table mode
+// checks lane-parallel.  Brackets inside strings count too: the key only orders the units, it never changes a result.
+static const uint32_t ORDER_WINDOW = 2048;   // bytes of a unit the key reads
+TP_FN uint32_t order_events(uint32_t prev, uint32_t w) {
+  const uint32_t p1 = (w << 8) | (prev >> 24), p2 = (w << 16) | (prev >> 16), p3 = (w << 24) | (prev >> 8);   // byte j <- byte j-1, j-2, j-3
+  const uint32_t open = swar_eq(w | 0x20202020u, '{');                                  // '{' or '[' ('[' | 0x20 == '{')
+  const uint32_t close_comma = swar_eq(p2, '}') & swar_eq(p1, ',');
+  const uint32_t row = swar_eq(w, '{') & (close_comma | (swar_eq(p3, '}') & swar_eq(p2, ',') & swar_eq(p1, ' ')));
+  return tpw::popc(open) - tpw::popc(row);
+}
+
 struct LaneMasks { uint32_t q, bs, ob, cb, curly, cm, co, ws, ctrl, hi, special, nonkey, digit; };   // bit j <-> byte j of the lane's 32 bytes
 TP_FN void build_masks(const uint32_t* w, LaneMasks& M) {
   M.q = M.bs = M.ob = M.cb = M.curly = M.cm = M.co = M.ws = M.ctrl = M.hi = M.special = M.nonkey = M.digit = 0;

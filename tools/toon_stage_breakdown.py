@@ -1,7 +1,8 @@
 """Where the TOON stage's time goes, by payload shape: cf_toon on a device-resident batch of bench.py's payloads.
 
 For each case (shapes A tabular, B nested config, P prose-in-JSON alone, each tiled from bench.make_payloads()'s own payloads of
-that shape, and the bench mix itself) it times, with CUDA events over warmed launches:
+that shape, the bench mix itself, and mix_sorted = the mix's texts packed by shape, B then A then P) it times, with CUDA events over
+warmed launches:
   flags = 0                the whole stage: token-parallel kernel + the sequential encoder for the units it hands over
   CF_TOON_NO_HANDOVER      the token-parallel kernel alone; the difference is the hand-over tail
 and reports median / min / max in ms, and how many units the token-parallel kernel handed over.
@@ -88,11 +89,15 @@ def main():
     by_shape = {}
     for i, p in enumerate(payloads):
         by_shape.setdefault(shape_of(i), []).append(p)
-    cases = {"A": by_shape["A"], "B": by_shape["B"], "P": by_shape["C"], "mix": payloads}
+    cases = {name: [base[i % len(base)] for i in range(args.units)]
+             for name, base in (("A", by_shape["A"]), ("B", by_shape["B"]), ("P", by_shape["C"]), ("mix", payloads))}
+    # the mix's own texts packed by shape, nested configs first: what the first pass costs when no CTA mixes shapes
+    rank = {"B": 0, "A": 1, "C": 2}
+    cases["mix_sorted"] = [payloads[i % len(payloads)]
+                           for i in sorted(range(args.units), key=lambda i: rank[shape_of(i % len(payloads))])]
     out = {"card": card(), "cases": {}}
     print(json.dumps(out["card"]))
-    for name, base in cases.items():
-        texts = [base[i % len(base)] for i in range(args.units)]
+    for name, texts in cases.items():
         r = time_case(ctx, texts, args.reps)
         out["cases"][name] = r
         print(f"{name:4s} units {r['units']}  stage {r['stage']['median_ms']:.3f} ms [{r['stage']['min_ms']:.3f}, {r['stage']['max_ms']:.3f}]  "
