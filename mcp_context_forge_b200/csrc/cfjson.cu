@@ -97,20 +97,19 @@ __global__ void __launch_bounds__(128) json_index_kernel(const uint8_t* __restri
 // ------------------------------------------------------------------------------------------------
 // toon_encoder, token-parallel (csrc/json_tp.h): one WARP per unit, two passes over the unit's bytes (the second
 // one comes from L2), 8-byte tokens through HBM scratch, no DOM.  Units the fast path does not cover get status
-// TS_FALLBACK (reason in out_len) and are re-done by the sequential toon_kernel below (TOON_ONLY_FALLBACK).  The units handed
-// over as mixed list-item arrays (FB_MIXED_ITEM) first get a second token-parallel pass that decides them (RESOLVE_PASS): it
-// costs key comparisons the first pass saves on every other unit, and a warp is far quicker than the sequential encoder's one
-// thread per unit.
-// The first pass takes its units in cost order (toon_order_kernel + a stable radix sort, heaviest first): a CTA holds its slot
+// TS_FALLBACK (reason in out_len) and are re-done by the sequential toon_kernel below (TOON_ONLY_FALLBACK).  A unit that stops
+// at a mixed list-item array (FB_MIXED_ITEM) is decided by the same warp right away: analyze in resolve mode and emit again over
+// the token array it already has (json_tp.h toon_unit).  Resolve mode costs key comparisons the first attempt saves on every
+// other unit, and a warp is far quicker than the sequential encoder's one thread per unit.
+// The kernel takes its units in cost order (toon_order_kernel + a stable radix sort, heaviest first): a CTA holds its slot
 // until its slowest warp is done, and a nested unit costs about three tabular ones, so CTAs that mix shapes idle most of their
-// warps.  In cost order each CTA, and at any moment each SM, runs units of one kind.  The resolving pass and the sequential
-// encoder keep the natural order: their few units are then spread over many SMs instead of packed into a few CTAs.
+// warps.  In cost order each CTA, and at any moment each SM, runs units of one kind.  The sequential encoder keeps the natural
+// order: its few units are then spread over many SMs instead of packed into a few CTAs.
 // ------------------------------------------------------------------------------------------------
 static const uint32_t TP_WARPS = 8;
 static const uint32_t TP_TOK_SLACK = 64;               // token capacity of unit u: len/2 + TP_TOK_SLACK
 static const uint32_t TP_WARP_SMEM = (uint32_t)sizeof(cftp::Shared) + cftp::STAGE;   // container stack + token ring | staging buffer
 static const uint32_t TP_SMEM = TP_WARPS * TP_WARP_SMEM;                              // 110 592 B: two CTAs per SM
-template <bool RESOLVE_PASS>
 __global__ void __launch_bounds__(TP_WARPS * 32, 2) toon_tp_kernel(const uint8_t* __restrict__ stream, const uint64_t* __restrict__ offsets, uint32_t n_units,
                                                                     cftp::GTok* __restrict__ toks, uint8_t* __restrict__ out, uint32_t* __restrict__ out_len,
                                                                     int32_t* __restrict__ status, uint32_t flags, const uint8_t* __restrict__ unit_stages,
@@ -119,9 +118,8 @@ __global__ void __launch_bounds__(TP_WARPS * 32, 2) toon_tp_kernel(const uint8_t
   const uint32_t lane = threadIdx.x & 31, wic = threadIdx.x >> 5;
   const uint32_t slot = blockIdx.x * TP_WARPS + wic;
   if (slot >= n_units) return;
-  const uint32_t u = RESOLVE_PASS ? slot : order[slot];
-  if (RESOLVE_PASS) { if (status[u] != cftp::TS_FALLBACK || out_len[u] != cftp::FB_MIXED_ITEM) return; }
-  else if (unit_stages && !(unit_stages[u] & CF_STAGE_TOON)) { if (lane == 0) { status[u] = CF_TOON_SKIPPED; out_len[u] = 0; } return; }
+  const uint32_t u = order[slot];
+  if (unit_stages && !(unit_stages[u] & CF_STAGE_TOON)) { if (lane == 0) { status[u] = CF_TOON_SKIPPED; out_len[u] = 0; } return; }
   cftp::Shared& sh = *reinterpret_cast<cftp::Shared*>(tp_smem + (size_t)wic * TP_WARP_SMEM);
   uint8_t* stage = tp_smem + (size_t)wic * TP_WARP_SMEM + sizeof(cftp::Shared);
   if (lane == 0) {                                   // the warp's mbarrier for its bulk TMA loads into the staging buffer
@@ -136,7 +134,9 @@ __global__ void __launch_bounds__(TP_WARPS * 32, 2) toon_tp_kernel(const uint8_t
   const uint32_t len = (uint32_t)len64;
   cftp::GTok* my = toks + (b >> 1) + (uint64_t)TP_TOK_SLACK * u;
   uint32_t ol = 0;
-  const int st = cftp::toon_unit_t<RESOLVE_PASS>(stream + b, len, my, len / 2 + TP_TOK_SLACK, out + b, len ? len - 1 : 0, &ol, sh, stage, (flags & 1u) != 0);
+  // CF_TOON_NO_HANDOVER: the first attempt only, so that a mixed list-item array still reports FB_MIXED_ITEM
+  const int st = cftp::toon_unit(stream + b, len, my, len / 2 + TP_TOK_SLACK, out + b, len ? len - 1 : 0, &ol, sh, stage, (flags & 1u) != 0,
+                                 !(flags & CF_TOON_NO_HANDOVER));
   if (lane == 0) {
     status[u] = st & 0xFF;
     out_len[u] = (st & 0xFF) == cfj::TS_CONVERTED ? ol : (uint32_t)st >> 8;
@@ -283,8 +283,7 @@ static int toon_launch(cf_ctx* ctx, cf_batch* b, uint32_t flags, uint8_t* d_out,
   if (tp) {
     static bool smem_set = false;
     if (!smem_set) {
-      CF_CUDA(ctx, cudaFuncSetAttribute(toon_tp_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TP_SMEM));
-      CF_CUDA(ctx, cudaFuncSetAttribute(toon_tp_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TP_SMEM));
+      CF_CUDA(ctx, cudaFuncSetAttribute(toon_tp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TP_SMEM));
       smem_set = true;
     }
     uint8_t* srt = (uint8_t*)ctx->toon_sort.p;
@@ -295,16 +294,10 @@ static int toon_launch(cf_ctx* ctx, cf_batch* b, uint32_t flags, uint8_t* d_out,
     CF_CUDA(ctx, cub::DeviceRadixSort::SortPairsDescending(srt + o_tmp, sort_tmp, srt + o_kin, srt + o_kout, (const uint32_t*)srt, order, (int)b->n, 0, 8, st));
     ctx->launches++;
     const uint32_t grid = (b->n + TP_WARPS - 1) / TP_WARPS;
-    toon_tp_kernel<false><<<grid, TP_WARPS * 32, TP_SMEM, st>>>(b->d_buf + cf::FRONT_PAD, b->d_offsets, b->n, (cftp::GTok*)ctx->d_toon_scratch, d_out, d_out_len,
-                                                                d_status, flags, d_unit_stages, order);
+    toon_tp_kernel<<<grid, TP_WARPS * 32, TP_SMEM, st>>>(b->d_buf + cf::FRONT_PAD, b->d_offsets, b->n, (cftp::GTok*)ctx->d_toon_scratch, d_out, d_out_len,
+                                                         d_status, flags, d_unit_stages, order);
     ctx->launches++;
     CF_CUDA(ctx, cudaGetLastError());
-    if (!(flags & CF_TOON_NO_HANDOVER)) {
-      toon_tp_kernel<true><<<grid, TP_WARPS * 32, TP_SMEM, st>>>(b->d_buf + cf::FRONT_PAD, b->d_offsets, b->n, (cftp::GTok*)ctx->d_toon_scratch, d_out, d_out_len,
-                                                                 d_status, flags, d_unit_stages, nullptr);
-      ctx->launches++;
-      CF_CUDA(ctx, cudaGetLastError());
-    }
     // the units the fast path handed over: sequential encoder, one unit per warp (they are few)
     if (!(flags & CF_TOON_NO_HANDOVER)) cf_launch_toon_seq(json_blocks(b->n, 1), st, b->d_buf + cf::FRONT_PAD, b->d_offsets, b->n, (cfj::JNode*)ctx->d_toon_scratch, d_out, d_out_len, d_status,
                                                      (flags & 1u) | TOON_ONLY_FALLBACK, 1);

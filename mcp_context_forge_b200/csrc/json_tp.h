@@ -1363,29 +1363,48 @@ TP_FN int emit(const uint8_t* s, const GTok* toks, uint32_t ntok, uint8_t* out, 
   return TS_CONVERTED;
 }
 
-// Whole per-unit pipeline (all 32 lanes call it with the same arguments).  out_cap = n - 1 in the product (a
-// conversion is only kept when strictly smaller).  Returns a TS_* status, TS_FALLBACK (| reason << 8) when the sequential
-// encoder has to redo the unit.
-// `stage` = STAGE bytes of per-warp scratch, 16-byte aligned (shared memory on the GPU).
+// analyze + emit over the token array tokenize produced.
 // RESOLVE_MIXED: decide mixed list-item arrays whose first row is not simple (C_R0KEYS) instead of returning FB_MIXED_ITEM.  Its key
-// bookkeeping would slow every nested unit down, so the first pass over a batch is compiled without it and a second pass with it runs
-// over the units that came back with FB_MIXED_ITEM only.
+// bookkeeping would slow every nested unit down, so a unit is first analyzed without it, and with it only when that attempt stops at
+// such an array (toon_unit's retry).
 template <bool RESOLVE_MIXED>
-TP_FN int toon_unit_t(const uint8_t* s, uint32_t n, GTok* toks, uint32_t tok_cap, uint8_t* out, uint32_t out_cap, uint32_t* out_len, Shared& sh,
+TP_FN int toon_tokens(const uint8_t* s, GTok* toks, uint32_t ntok, uint32_t tok_cap, uint8_t* out, uint32_t out_cap, uint32_t* out_len, Shared& sh,
                       uint8_t* stage, bool report_errors) {
-  uint32_t ntok = 0;
-  int st = tokenize(s, n, toks, tok_cap, sh, stage, &ntok);
-  if (st) return st;
-  tpw::sync();
-  st = analyze<RESOLVE_MIXED>(s, toks, ntok, tok_cap, sh, stage);
+  const int st = analyze<RESOLVE_MIXED>(s, toks, ntok, tok_cap, sh, stage);
   if (st) return st;
   tpw::sync();
   return emit(s, toks, ntok, out, out_cap, out_len, sh, stage, report_errors);
 }
+// The retry in resolve mode, out of line: 2 % of the bench mix's units take it, and inlined beside the first attempt it made the tabular and
+// prose units' code larger and those shapes slower (DESIGN.md §6).
+TP_SLOW int toon_tokens_resolve(const uint8_t* s, GTok* toks, uint32_t ntok, uint32_t tok_cap, uint8_t* out, uint32_t out_cap, uint32_t* out_len,
+                                Shared& sh, uint8_t* stage, bool report_errors) {
+  return toon_tokens<true>(s, toks, ntok, tok_cap, out, out_cap, out_len, sh, stage, report_errors);
+}
+
+// Whole per-unit pipeline (all 32 lanes call it with the same arguments).  out_cap = n - 1 in the product (a
+// conversion is only kept when strictly smaller).  Returns a TS_* status, TS_FALLBACK (| reason << 8) when the sequential
+// encoder has to redo the unit.
+// `stage` = STAGE bytes of per-warp scratch, 16-byte aligned (shared memory on the GPU).
+// retry_mixed: a unit whose first attempt stops at a mixed list-item array (exactly FB_MIXED_ITEM) is analyzed again in resolve mode
+// and emitted again, over the SAME token array.  That array is a valid input to a second analyze: analyze patches an opener from a
+// word it rebuilds out of the separator bits alone (gt_patch keeps them and replaces kind, flags and length), so a patched opener
+// reads as the tokenizer's; an_rows patches row openers the same way, and nothing else writes into the array after tokenize.
+// Every Shared field analyze reads was written earlier in the same walk, and every bulk copy into `stage` has completed when
+// stage_load returns, so the mbarrier's phase stays in step.  The failed emit's output is overwritten and out_len is set by a
+// successful emit only.
 TP_FN int toon_unit(const uint8_t* s, uint32_t n, GTok* toks, uint32_t tok_cap, uint8_t* out, uint32_t out_cap, uint32_t* out_len, Shared& sh,
-                    uint8_t* stage, bool report_errors, bool resolve_mixed = false) {
-  return resolve_mixed ? toon_unit_t<true>(s, n, toks, tok_cap, out, out_cap, out_len, sh, stage, report_errors)
-                       : toon_unit_t<false>(s, n, toks, tok_cap, out, out_cap, out_len, sh, stage, report_errors);
+                    uint8_t* stage, bool report_errors, bool retry_mixed = false) {
+  uint32_t ntok = 0;
+  int st = tokenize(s, n, toks, tok_cap, sh, stage, &ntok);
+  if (st) return st;
+  tpw::sync();
+  st = toon_tokens<false>(s, toks, ntok, tok_cap, out, out_cap, out_len, sh, stage, report_errors);
+  if (retry_mixed && st == (TS_FALLBACK | (int)(FB_MIXED_ITEM << 8))) {
+    tpw::sync();
+    st = toon_tokens_resolve(s, toks, ntok, tok_cap, out, out_cap, out_len, sh, stage, report_errors);
+  }
+  return st;
 }
 
 }  // namespace cftp

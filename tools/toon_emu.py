@@ -1,5 +1,6 @@
-"""ctypes access to tools/toon_emu.cpp: the token-parallel TOON kernel body on the CPU warp emulator, first pass and the resolving
-pass for mixed list-item arrays, as toon_tp_kernel runs them.  The library is compiled with g++ into a temporary directory on first use."""
+"""ctypes access to tools/toon_emu.cpp: the token-parallel TOON kernel body on the CPU warp emulator, as toon_tp_kernel runs it (the
+first attempt, and the in-place retry of a unit that stops at a mixed list-item array), plus the separate resolving pass that retry
+replaced.  The library is compiled with g++ into a temporary directory on first use."""
 import ctypes
 import os
 import subprocess
@@ -8,6 +9,7 @@ import tempfile
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SRCS = [os.path.join(ROOT, "tools", "toon_emu.cpp"), os.path.join(ROOT, "tests", "hostsim", "warp_emu.cpp")]
 FB_MIXED_ITEM, TS_FALLBACK = 7, 7
+FIRST, RESOLVE, IN_PLACE = 0, 1, 2          # toon_emu.cpp's modes
 _lib = None
 
 
@@ -20,22 +22,25 @@ def lib():
     return _lib
 
 
-def toon_pass(text, resolve_mixed: bool, unlimited: bool = False, report_errors: bool = True, order: int = 0):
-    """One pass: (status, toon_text_or_None, fallback reason, warp collectives)."""
+def run(text, mode: int, unlimited: bool = False, report_errors: bool = True, order: int = 0):
+    """One emulated run in toon_emu.cpp's `mode`: (status, toon_text_or_None, fallback reason, out_len, warp collectives)."""
     b = text if isinstance(text, bytes) else text.encode("utf-8", "surrogatepass")
     cap = len(b) * 6 + 4096 if unlimited else max(len(b) - 1, 0)
     out = ctypes.create_string_buffer(max(cap, 1))
     n, why, coll = ctypes.c_uint32(), ctypes.c_uint32(), ctypes.c_ulonglong()
-    st = lib().toon_emu_unit(b, len(b), out, cap, ctypes.byref(n), 1 if report_errors else 0, order, 1 if resolve_mixed else 0, ctypes.byref(why),
-                             ctypes.byref(coll))
+    st = lib().toon_emu_unit(b, len(b), out, cap, ctypes.byref(n), 1 if report_errors else 0, order, mode, ctypes.byref(why), ctypes.byref(coll))
     assert st >= 0, st
-    return st, (out.raw[: n.value].decode("utf-8", "surrogatepass") if st == 0 else None), why.value, coll.value
+    return st, (out.raw[: n.value].decode("utf-8", "surrogatepass") if st == 0 else None), why.value, n.value, coll.value
+
+
+def toon_pass(text, resolve_mixed: bool, **kw):
+    """One pass over the unit from its bytes, the first attempt or the resolving pass: (status, toon_text_or_None, fallback reason,
+    warp collectives)."""
+    st, txt, why, _, coll = run(text, RESOLVE if resolve_mixed else FIRST, **kw)
+    return st, txt, why, coll
 
 
 def toon_tp(text, **kw):
-    """Both passes as on the device: (status, text, reason, collectives of the first pass, collectives of the resolving pass or 0)."""
-    st, txt, why, c1 = toon_pass(text, False, **kw)
-    if st == TS_FALLBACK and why == FB_MIXED_ITEM:
-        st, txt, why, c2 = toon_pass(text, True, **kw)
-        return st, txt, why, c1, c2
-    return st, txt, why, c1, 0
+    """The unit as toon_tp_kernel encodes it, a mixed list-item array retried in place: (status, toon_text_or_None, fallback reason,
+    out_len, warp collectives)."""
+    return run(text, IN_PLACE, **kw)

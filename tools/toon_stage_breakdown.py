@@ -3,8 +3,10 @@
 For each case (shapes A tabular, B nested config, P prose-in-JSON alone, each tiled from bench.make_payloads()'s own payloads of
 that shape, the bench mix itself, and mix_sorted = the mix's texts packed by shape, B then A then P) it times, with CUDA events over
 warmed launches:
-  flags = 0                the whole stage: token-parallel kernel + the sequential encoder for the units it hands over
-  CF_TOON_NO_HANDOVER      the token-parallel kernel alone; the difference is the hand-over tail
+  flags = 0                the whole stage: token-parallel kernel (mixed list-item arrays retried in place) + the sequential encoder for
+                           the units it hands over
+  CF_TOON_NO_HANDOVER      the token-parallel kernel alone, first attempts only; the difference is the hand-over tail: the sequential
+                           encoder's launch, plus the in-place retries' share of the kernel
 and reports median / min / max in ms, and how many units the token-parallel kernel handed over.
 
 usage: python tools/toon_stage_breakdown.py [--units 32768] [--reps 15] [--json OUT]
