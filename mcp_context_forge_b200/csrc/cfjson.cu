@@ -109,8 +109,13 @@ __global__ void __launch_bounds__(128) json_index_kernel(const uint8_t* __restri
 static const uint32_t TP_WARPS = 8;
 static const uint32_t TP_TOK_SLACK = 64;               // token capacity of unit u: len/2 + TP_TOK_SLACK
 static const uint32_t TP_WARP_SMEM = (uint32_t)sizeof(cftp::Shared) + cftp::STAGE;   // container stack + token ring | staging buffer
-static const uint32_t TP_SMEM = TP_WARPS * TP_WARP_SMEM;                              // 110 592 B: two CTAs per SM
-__global__ void __launch_bounds__(TP_WARPS * 32, 2) toon_tp_kernel(const uint8_t* __restrict__ stream, const uint64_t* __restrict__ offsets, uint32_t n_units,
+// Three CTAs (24 warps) per SM: the kernel is latency-bound (a warp works through its unit in serial, dependent steps), so
+// resident warps are what hides the latency.  That needs <= 80 registers per thread and <= 75 KB of shared memory per CTA
+// (3 x (75 904 + 1 024 reserved) B of the SM's 228 KB); tests/test_toon_occupancy_cpu.py holds both.
+static const uint32_t TP_CTAS_PER_SM = 3;
+static const uint32_t TP_SMEM = TP_WARPS * TP_WARP_SMEM;                              // 75 904 B
+static_assert(TP_CTAS_PER_SM * (TP_SMEM + 1024) <= 228 * 1024, "TP_CTAS_PER_SM CTAs fit the SM's shared memory");
+__global__ void __launch_bounds__(TP_WARPS * 32, TP_CTAS_PER_SM) toon_tp_kernel(const uint8_t* __restrict__ stream, const uint64_t* __restrict__ offsets, uint32_t n_units,
                                                                     cftp::GTok* __restrict__ toks, uint8_t* __restrict__ out, uint32_t* __restrict__ out_len,
                                                                     int32_t* __restrict__ status, uint32_t flags, const uint8_t* __restrict__ unit_stages,
                                                                     const uint32_t* __restrict__ order) {
@@ -332,6 +337,14 @@ int cf_chain(cf_ctx* ctx, cf_prog* prog, cf_batch* b, uint32_t stage_mask, uint3
     if ((rc = toon_launch(ctx, b, toon_flags, d_out, d_out_len, d_status, d_unit_stages, (cudaStream_t)cuda_stream))) return rc;
   }
   return CF_OK;
+}
+
+// Not part of the C API (include/cfgpu.h): the token-parallel kernel's launch shape for tests/test_toon_occupancy_cpu.py, which
+// checks it against the built kernel's resource usage without a device.
+void cf_toon_tp_config(uint32_t* warps_per_cta, uint32_t* ctas_per_sm, uint32_t* smem_per_cta) {
+  if (warps_per_cta) *warps_per_cta = TP_WARPS;
+  if (ctas_per_sm) *ctas_per_sm = TP_CTAS_PER_SM;
+  if (smem_per_cta) *smem_per_cta = TP_SMEM;
 }
 
 int cf_toon_host(cf_ctx* ctx, cf_batch* b, uint32_t flags, const uint8_t* stream, uint64_t stream_bytes, const uint64_t* offsets,

@@ -63,22 +63,27 @@ enum : uint32_t { RM_KIND = 7u, RM_NCOMMA_SH = 3, RM_NCOLON_SH = 5, RM_SPECIAL =
                   RM_ALLDIGIT = 1u << 12 /* scalar run consists of ASCII digits only */ };
 
 // ---- per-warp shared memory ----------------------------------------------------------------------------------------
+// Shared + the staging buffer (STAGE) is what one warp owns: 9 488 B, so that three 8-warp CTAs fit an SM (cfjson.cu TP_SMEM).
+// Storage no two phases use at once is shared: tokenize keeps its ring's meta words behind the source window in the staging
+// buffer, and emit's table rounds stage their output over the analyze-only fields (row_out).
 static const uint32_t RING = 256, MAXD = 64, KH_CAP = 256;
 static const uint32_t TOK_WIN = 192;      // tokens of one 1 KiB step pushed through the ring at a time (a window never overtakes the 32-token batches)
 static const uint32_t UNSET = 0xFFFFFFFFu;
 struct Shared {
-  uint32_t ring_pos[RING], ring_len[RING], ring_meta[RING];   // tokenize | analyze: ring_pos[j], ring_len[j] = the key whose hash is kh[j]
+  unsigned long long sbar_bar;         // mbarrier of the staging buffer's bulk TMA loads (initialised by the kernel)
+  uint32_t sbar_phase, sbar_pad;
   // analyze: container stack            | emit: frame stack (same storage)
   uint32_t open_idx[MAXD];             // token index of the opener      | frame mode
   uint32_t cnt[MAXD];                  // children (values) so far       | children so far
   uint32_t cfl[MAXD];                  // C_* flags                      | prefix width
   uint32_t khbase[MAXD];               // base of the key hashes         | indent level
+  // tokenize and analyze only: from row0_idx to the end, emit's table rounds stage their output here (row_out)
   uint32_t row0_idx[MAXD];             // arrays: 1 + token index of the first element when it is an object
   uint32_t row0_n[MAXD];               // arrays: member count of that first object once it closed
-  uint32_t kh[KH_CAP];                 // key hashes of the open objects (stack)
   uint32_t open_w[MAXD];               // analyze: the opener's token word (its separator bits survive the patch)
-  unsigned long long sbar_bar;         // mbarrier of the staging buffer's bulk TMA loads (initialised by the kernel)
-  uint32_t sbar_phase, sbar_pad;
+  uint32_t kh[KH_CAP];                 // key hashes of the open objects (stack)
+  uint32_t ring_pos[RING], ring_len[RING];   // tokenize | analyze: ring_pos[j], ring_len[j] = the key whose hash is kh[j]
+  TP_FN uint8_t* row_out() { return reinterpret_cast<uint8_t*>(row0_idx); }
 };
 enum : uint32_t {
   C_OBJ = 1,
@@ -104,9 +109,14 @@ enum : uint32_t {
 // Per-warp staging buffer (shared memory on the GPU): lane-strided byte accesses to global memory cost one L1 wavefront per
 // lane (profiles/r02_toon_tp_v2_ncu.txt: the kernel was bound by exactly that), so whatever a lane reads byte by byte is
 // first brought in with coalesced 16-byte loads, and table rows are written to global memory through it the same way.
-static const uint32_t STAGE = 8192;          // bytes per warp
-static const uint32_t WIN = 2048;            // tokenizer: the last two 1 KiB steps of source text
-static const uint32_t ROW_SRC = 5120, ROW_OUT = STAGE - ROW_SRC;   // table rows: source bytes of a round | its output
+static const uint32_t STAGE = 4608;          // bytes per warp
+static const uint32_t WIN = 2048;            // tokenizer: the last two 1 KiB steps of source text, then the ring's meta words (RING of them)
+// table rows: source bytes of a round (the staging buffer) | its output (Shared::row_out, 3 840 B); an A-shaped row of ~150 source
+// bytes writes ~95, so a round of 30 rows fits both
+static const uint32_t ROW_SRC = STAGE, ROW_OUT = (uint32_t)(sizeof(Shared) - 16 - 4 * 4 * MAXD);
+static_assert(WIN + 4 * RING <= STAGE, "tokenizer window + ring meta fit the staging buffer");
+static_assert(ROW_OUT == 3 * 4 * MAXD + 4 * KH_CAP + 2 * 4 * RING, "row_out spans row0_idx .. the end of Shared");
+static_assert(sizeof(Shared) % 16 == 0 && (16 + 4 * 4 * MAXD) % 16 == 0, "row_out and the staging buffer behind Shared stay 16-byte aligned");
 
 // stage[0..) <- s[a0 .. a1) where a0 is rounded down to the 16-byte grid; returns the unit position of stage[0] (can be negative)
 // On the GPU the copy is ONE bulk TMA transfer (cp.async.bulk global -> shared, SASS UBLKCP) completing on the warp's mbarrier.
@@ -467,6 +477,9 @@ TP_SLOW uint32_t warp_escapes(const uint8_t* s, uint32_t a, uint32_t len) {
 // front of the token that follows the batch (a string followed by a colon is a key)
 // ----------------------------------------------------------------------------------------------------------------------
 struct TokState { uint32_t ntok; int status; };
+// the ring's meta words live behind the tokenizer's source window in the staging buffer (its positions and lengths in Shared)
+TP_FN uint32_t* ring_meta(uint8_t* stage) { return reinterpret_cast<uint32_t*>(stage + WIN); }
+TP_FN const uint32_t* ring_meta(const uint8_t* stage) { return reinterpret_cast<const uint32_t*>(stage + WIN); }
 // win[0..WIN) holds the unit's bytes [wlo, wlo + WIN) (unit positions; wlo may be "negative" = wrapped, see in_window)
 TP_FN const uint8_t* in_window(const uint8_t* s, const uint8_t* win, uint32_t wlo, uint32_t pos, uint32_t len) {
   const uint32_t d = pos - wlo;                       // wraps to a huge value when pos < wlo
@@ -477,7 +490,7 @@ TP_FN void tok_batch(const uint8_t* s, uint32_t n, GTok* toks, uint32_t tok_cap,
   const uint32_t l = tpw::lane();
   const bool act = l < m;
   uint32_t pos = 0, len = 0, meta = 0;
-  if (act) { const uint32_t r = (head + l) & (RING - 1); pos = sh.ring_pos[r]; len = sh.ring_len[r]; meta = sh.ring_meta[r]; }
+  if (act) { const uint32_t r = (head + l) & (RING - 1); pos = sh.ring_pos[r]; len = sh.ring_len[r]; meta = ring_meta(win)[r]; }
   uint32_t kind = meta & RM_KIND;
   const uint32_t ncomma = (meta >> RM_NCOMMA_SH) & 3u, ncolon = (meta >> RM_NCOLON_SH) & 3u;
   uint32_t nxt_ncolon = tpw::shfl_down(ncolon, 1);
@@ -590,26 +603,24 @@ TP_FN int tokenize(const uint8_t* s, uint32_t n, GTok* toks, uint32_t tok_cap, S
   const uint32_t l = tpw::lane();
   const uint32_t ltm = tpw::lt_mask();
   TokState st; st.ntok = 0; st.status = 0;
+  uint32_t* rmeta = ring_meta(stage);
   const uint32_t lead = (uint32_t)((uintptr_t)s & 15u);
   const uint8_t* s0 = s - lead;                       // 16-byte aligned
   const uint32_t vend = n + lead;
-  // carries between steps (warp-uniform)
-  uint32_t c_instr = 0, c_esc = 0, c_other = 0, c_sep = 0 /* commas | colons << 16 since the last token */;
-  uint32_t c_open = 0, c_cls = 0;                     // string open across steps: position of its opening quote, classes seen so far
+  // carries between steps (warp-uniform), the one-bit ones and the open string's classes packed into one word (registers are what
+  // limits the resident warps): bit 0 inside a string, bit 1 the next byte is escaped, bit 2 a scalar run continues, bits 4..7 classes
+  uint32_t c_bits = 0, c_sep = 0 /* commas | colons << 16 since the last token */;
+  uint32_t c_open = 0;                                // string open across steps: position of its opening quote
   uint32_t head = 0, rcount = 0;
   for (uint32_t vb = 0; vb < vend; vb += 1024) {
     const uint32_t v = vb + 32 * l;                   // virtual offset of this lane's first byte
     uint32_t w[8];
-    uint32_t valid = 0xFFFFFFFFu;
     if (v < vend) {
       const uint4 a = *reinterpret_cast<const uint4*>(s0 + v), b = *reinterpret_cast<const uint4*>(s0 + v + 16);
       w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w; w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
-      if (v < lead) valid &= ~bits_below(lead - v);
-      if (v + 32 > vend) valid &= bits_below(vend - v);
     } else {
 #pragma unroll
       for (uint32_t k = 0; k < 8; ++k) w[k] = 0x20202020u;
-      valid = 0;
     }
     // source window for the classification batches: [previous step | this step]
     {
@@ -622,162 +633,181 @@ TP_FN int tokenize(const uint8_t* s, uint32_t n, GTok* toks, uint32_t tok_cap, S
       tpw::sync();
     }
     const uint32_t wlo = vb - 1024 - lead;             // unit position of stage[0] (wraps for the first step: nothing lies there)
-    LaneMasks M;
-    build_masks(w, M);
-    if (valid != 0xFFFFFFFFu) {
-      M.q &= valid; M.bs &= valid; M.ob &= valid; M.cb &= valid; M.curly &= valid; M.cm &= valid; M.co &= valid; M.ctrl &= valid; M.hi &= valid;
-      M.special &= valid; M.nonkey &= valid; M.digit &= valid; M.ws |= ~valid;
-    }
-    // ---- escapes: which quotes are real
-    uint32_t quotes = M.q;
-    if (tpw::any(M.bs != 0) || c_esc) {
-      uint32_t eo;
-      find_escaped(M.bs, 0, &eo);
-      uint32_t e_in = tpw::shfl_up(eo, 1);
-      if (l == 0) e_in = c_esc;
-      if (tpw::any(M.bs == 0xFFFFFFFFu)) {            // a whole lane of backslashes: its carry-out depends on its carry-in
-        uint32_t e = c_esc;
-        for (uint32_t k = 0; k < 32; ++k) {
-          const uint32_t bk = tpw::shfl(M.bs, k);
-          uint32_t ek;
-          find_escaped(bk, e, &ek);
-          if (l == k) e_in = e;
-          e = ek;
+    // The step's masks are rebuilt for every window of TOK_WIN tokens, from its bytes in the staging buffer and the carries at the
+    // step's start, so that none of them is live across the classification batches (tok_batch): 80 registers hold either, not both.
+    // A step with more than one window (over TOK_WIN tokens in 1 KiB) is rare; it pays the mask algebra once more per window.
+    const uint32_t c_bits0 = c_bits, c_sep0 = c_sep, c_open0 = c_open;
+    for (uint32_t done = 0;; done += TOK_WIN) {
+      c_bits = c_bits0; c_sep = c_sep0; c_open = c_open0;
+      {
+        const uint4 a = *reinterpret_cast<const uint4*>(stage + 1024 + 32 * l), b = *reinterpret_cast<const uint4*>(stage + 1024 + 32 * l + 16);
+        w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w; w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
+      }
+      uint32_t valid = 0;
+      if (v < vend) {
+        valid = 0xFFFFFFFFu;
+        if (v < lead) valid &= ~bits_below(lead - v);
+        if (v + 32 > vend) valid &= bits_below(vend - v);
+      }
+      LaneMasks M;
+      build_masks(w, M);
+      if (valid != 0xFFFFFFFFu) {
+        M.q &= valid; M.bs &= valid; M.ob &= valid; M.cb &= valid; M.curly &= valid; M.cm &= valid; M.co &= valid; M.ctrl &= valid; M.hi &= valid;
+        M.special &= valid; M.nonkey &= valid; M.digit &= valid; M.ws |= ~valid;
+      }
+      // ---- escapes: which quotes are real
+      uint32_t quotes = M.q;
+      if (tpw::any(M.bs != 0) || (c_bits & 2u)) {
+        uint32_t eo;
+        find_escaped(M.bs, 0, &eo);
+        uint32_t e_in = tpw::shfl_up(eo, 1);
+        if (l == 0) e_in = (c_bits >> 1) & 1u;
+        if (tpw::any(M.bs == 0xFFFFFFFFu)) {            // a whole lane of backslashes: its carry-out depends on its carry-in
+          uint32_t e = (c_bits >> 1) & 1u;
+          for (uint32_t k = 0; k < 32; ++k) {
+            const uint32_t bk = tpw::shfl(M.bs, k);
+            uint32_t ek;
+            find_escaped(bk, e, &ek);
+            if (l == k) e_in = e;
+            e = ek;
+          }
         }
+        uint32_t eo2;
+        const uint32_t escaped = find_escaped(M.bs, e_in, &eo2);
+        quotes &= ~escaped;
+        c_bits = (c_bits & ~2u) | (tpw::shfl(eo2, 31) << 1);
       }
-      uint32_t eo2;
-      const uint32_t escaped = find_escaped(M.bs, e_in, &eo2);
-      quotes &= ~escaped;
-      c_esc = tpw::shfl(eo2, 31);
-    }
-    // ---- in-string state
-    const uint32_t par = tpw::ballot(tpw::popc(quotes) & 1u);
-    const uint32_t is_in = (c_instr ^ (tpw::popc(par & ltm) & 1u)) ? 0xFFFFFFFFu : 0u;   // this lane starts inside a string
-    c_instr ^= tpw::popc(par) & 1u;
-    uint32_t x = quotes;
-    x ^= x << 1; x ^= x << 2; x ^= x << 4; x ^= x << 8; x ^= x << 16;
-    const uint32_t instr = x ^ is_in;                 // opening quote included, closing quote excluded
-    const uint32_t openq = quotes & instr, closeq = quotes & ~instr;
-    const uint32_t content = instr & ~openq;
-    const bool ctl_bad = (M.ctrl & content) != 0;      // raw control character inside a string
-    const uint32_t outside = ~instr & ~closeq;
-    const uint32_t st_all = M.ob | M.cb | M.cm | M.co;
-    const uint32_t comma_out = M.cm & outside, colon_out = M.co & outside;
-    const uint32_t other = outside & ~st_all & ~M.ws;
-    uint32_t prev_other = tpw::shfl_up(other >> 31, 1);
-    if (l == 0) prev_other = c_other;
-    c_other = tpw::shfl(other >> 31, 31);
-    const uint32_t starts = other & ~((other << 1) | prev_other);
-    const uint32_t brackets = (M.ob | M.cb) & outside;
-    const uint32_t T = brackets | closeq | starts;
-    if (tpw::any(ctl_bad)) { st.status = TS_NOT_JSON; break; }
-    const uint32_t m_special = M.special & content, m_nonkey = M.nonkey & content, m_hi = M.hi & content, m_bs = M.bs & content;
-    // ---- separators in front of each lane's first token: segmented scan over the lanes
-    uint32_t sep_in;
-    {
-      const uint32_t after = T ? ~bits_below(32 - tpw::clz(T)) : 0xFFFFFFFFu;
-      uint32_t r = T ? 1u : 0u, vv = tpw::popc(comma_out & after) | (tpw::popc(colon_out & after) << 16);
-#pragma unroll
-      for (uint32_t d = 1; d < 32; d <<= 1) {
-        const uint32_t r2 = tpw::shfl_up(r, d), v2 = tpw::shfl_up(vv, d);
-        if (l >= d) { if (!r) vv += v2; r |= r2; }
+      // ---- in-string state
+      const uint32_t par = tpw::ballot(tpw::popc(quotes) & 1u);
+      const uint32_t is_in = ((c_bits & 1u) ^ (tpw::popc(par & ltm) & 1u)) ? 0xFFFFFFFFu : 0u;   // this lane starts inside a string
+      c_bits ^= tpw::popc(par) & 1u;
+      uint32_t x = quotes;
+      x ^= x << 1; x ^= x << 2; x ^= x << 4; x ^= x << 8; x ^= x << 16;
+      const uint32_t instr = x ^ is_in;                 // opening quote included, closing quote excluded
+      const uint32_t openq = quotes & instr, closeq = quotes & ~instr;
+      const uint32_t content = instr & ~openq;
+      const bool ctl_bad = (M.ctrl & content) != 0;      // raw control character inside a string
+      const uint32_t outside = ~instr & ~closeq;
+      const uint32_t st_all = M.ob | M.cb | M.cm | M.co;
+      const uint32_t comma_out = M.cm & outside, colon_out = M.co & outside;
+      const uint32_t other = outside & ~st_all & ~M.ws;
+      uint32_t prev_other = tpw::shfl_up(other >> 31, 1);
+      if (l == 0) prev_other = (c_bits >> 2) & 1u;
+      c_bits = (c_bits & ~4u) | (tpw::shfl(other >> 31, 31) << 2);
+      const uint32_t starts = other & ~((other << 1) | prev_other);
+      const uint32_t brackets = (M.ob | M.cb) & outside;
+      const uint32_t T = brackets | closeq | starts;
+      if (tpw::any(ctl_bad)) { st.status = TS_NOT_JSON; break; }
+      const uint32_t m_special = M.special & content, m_nonkey = M.nonkey & content, m_hi = M.hi & content, m_bs = M.bs & content;
+      // ---- separators in front of each lane's first token: segmented scan over the lanes
+      uint32_t sep_in;
+      {
+        const uint32_t after = T ? ~bits_below(32 - tpw::clz(T)) : 0xFFFFFFFFu;
+        uint32_t r = T ? 1u : 0u, vv = tpw::popc(comma_out & after) | (tpw::popc(colon_out & after) << 16);
+  #pragma unroll
+        for (uint32_t d = 1; d < 32; d <<= 1) {
+          const uint32_t r2 = tpw::shfl_up(r, d), v2 = tpw::shfl_up(vv, d);
+          if (l >= d) { if (!r) vv += v2; r |= r2; }
+        }
+        uint32_t rin = tpw::shfl_up(r, 1), vin = tpw::shfl_up(vv, 1);
+        if (l == 0) { rin = 0; vin = 0; }
+        sep_in = vin + (rin ? 0u : c_sep);
+        const uint32_t r31 = tpw::shfl(r, 31), v31 = tpw::shfl(vv, 31);
+        c_sep = v31 + (r31 ? 0u : c_sep);
+        if ((c_sep & 0xFFFFu) > 3u) c_sep = (c_sep & 0xFFFF0000u) | 3u;
+        if ((c_sep >> 16) > 3u) c_sep = (c_sep & 0xFFFFu) | (3u << 16);
       }
-      uint32_t rin = tpw::shfl_up(r, 1), vin = tpw::shfl_up(vv, 1);
-      if (l == 0) { rin = 0; vin = 0; }
-      sep_in = vin + (rin ? 0u : c_sep);
-      const uint32_t r31 = tpw::shfl(r, 31), v31 = tpw::shfl(vv, 31);
-      c_sep = v31 + (r31 ? 0u : c_sep);
-      if ((c_sep & 0xFFFFu) > 3u) c_sep = (c_sep & 0xFFFF0000u) | 3u;
-      if ((c_sep >> 16) > 3u) c_sep = (c_sep & 0xFFFFu) | (3u << 16);
-    }
-    // ---- the string that is open at each lane's start: position of its opening quote + classes seen so far
-    uint32_t so_pos, so_cls;
-    {
-      uint32_t r = quotes ? 1u : 0u, pp = 0, cc;
-      if (quotes) {                                    // only meaningful when the lane ends inside a string it opened
-        const uint32_t ob = 31 - tpw::clz(quotes), after = ~bits_below(ob + 1);
-        pp = v + ob;
-        cc = ((m_special & after) ? 1u : 0u) | ((m_nonkey & after) ? 2u : 0u) | ((m_hi & after) ? 4u : 0u) | ((m_bs & after) ? 8u : 0u);
-      } else cc = (m_special ? 1u : 0u) | (m_nonkey ? 2u : 0u) | (m_hi ? 4u : 0u) | (m_bs ? 8u : 0u);
-#pragma unroll
-      for (uint32_t d = 1; d < 32; d <<= 1) {
-        const uint32_t r2 = tpw::shfl_up(r, d), p2 = tpw::shfl_up(pp, d), c2 = tpw::shfl_up(cc, d);
-        if (l >= d && !r) { pp = p2; cc |= c2; r = r2; }
+      // ---- the string that is open at each lane's start: position of its opening quote + classes seen so far
+      uint32_t so_pos, so_cls;
+      {
+        uint32_t r = quotes ? 1u : 0u, pp = 0, cc;
+        if (quotes) {                                    // only meaningful when the lane ends inside a string it opened
+          const uint32_t ob = 31 - tpw::clz(quotes), after = ~bits_below(ob + 1);
+          pp = v + ob;
+          cc = ((m_special & after) ? 1u : 0u) | ((m_nonkey & after) ? 2u : 0u) | ((m_hi & after) ? 4u : 0u) | ((m_bs & after) ? 8u : 0u);
+        } else cc = (m_special ? 1u : 0u) | (m_nonkey ? 2u : 0u) | (m_hi ? 4u : 0u) | (m_bs ? 8u : 0u);
+  #pragma unroll
+        for (uint32_t d = 1; d < 32; d <<= 1) {
+          const uint32_t r2 = tpw::shfl_up(r, d), p2 = tpw::shfl_up(pp, d), c2 = tpw::shfl_up(cc, d);
+          if (l >= d && !r) { pp = p2; cc |= c2; r = r2; }
+        }
+        uint32_t rin = tpw::shfl_up(r, 1), pin = tpw::shfl_up(pp, 1), cin = tpw::shfl_up(cc, 1);
+        if (l == 0) { rin = 0; pin = 0; cin = 0; }
+        so_pos = rin ? pin : c_open;
+        so_cls = rin ? cin : (cin | (c_bits >> 4));
+        const uint32_t r31 = tpw::shfl(r, 31), p31 = tpw::shfl(pp, 31), c31 = tpw::shfl(cc, 31);
+        if (!r31) c_bits |= c31 << 4; else { c_open = p31; c_bits = (c_bits & 15u) | (c31 << 4); }
       }
-      uint32_t rin = tpw::shfl_up(r, 1), pin = tpw::shfl_up(pp, 1), cin = tpw::shfl_up(cc, 1);
-      if (l == 0) { rin = 0; pin = 0; cin = 0; }
-      so_pos = rin ? pin : c_open;
-      so_cls = rin ? cin : (cin | c_cls);
-      const uint32_t r31 = tpw::shfl(r, 31), p31 = tpw::shfl(pp, 31), c31 = tpw::shfl(cc, 31);
-      if (!r31) c_cls |= c31; else { c_open = p31; c_cls = c31; }
-    }
-    // ---- tokens of this lane through the ring (TOK_WIN at a time), one pass per token kind so that the lanes of a pass
-    // run the same code: slot = rank of the token in text order, separators = commas / colons since the previous token
-    const uint32_t cntT = tpw::popc(T);
-    const uint32_t incl = tpw::scan_incl(cntT);
-    const uint32_t lane_off = incl - cntT, total = tpw::shfl(incl, 31);
-    uint32_t other_nx = tpw::shfl_down(other, 1);       // the next lane's scalar bytes: a run may continue there
-    if (l == 31) other_nx = 0xFFFFFFFFu;                // unknown: treated as "continues" -> RM_OPENEND
-    for (uint32_t done = 0; done < total && !st.status; done += TOK_WIN) {
-      const uint32_t win = total - done > TOK_WIN ? TOK_WIN : total - done;
-      const uint32_t lo = done > lane_off ? done - lane_off : 0u, hi = done + win > lane_off ? done + win - lane_off : 0u;   // ranks [lo, hi) of this lane
-#define TP_TOKEN_PROLOGUE(MASK)                                                                               \
-      for (uint32_t tm = (MASK); tm;) {                                                                       \
-        const uint32_t j = tpw::ffs(tm) - 1;                                                                  \
-        tm &= tm - 1;                                                                                         \
-        const uint32_t below = bits_below(j), rank = tpw::popc(T & below);                                    \
-        if (rank < lo || rank >= hi) continue;                                                                \
-        const uint32_t pt = T & below;                                                                        \
-        uint32_t between = below, nc = sep_in & 0xFFFFu, nk = sep_in >> 16;                                   \
-        if (pt) { between = below & ~bits_below(32 - tpw::clz(pt)); nc = 0; nk = 0; }                         \
-        nc = sat3(nc + tpw::popc(comma_out & between));                                                       \
-        nk = sat3(nk + tpw::popc(colon_out & between));                                                       \
-        uint32_t meta = (nc << RM_NCOMMA_SH) | (nk << RM_NCOLON_SH), tpos = v + j - lead, tlen = 0;           \
-        const uint32_t r = (head + rcount + (lane_off + rank - done)) & (RING - 1);
-#define TP_TOKEN_EPILOGUE                                                                                     \
-        sh.ring_pos[r] = tpos; sh.ring_len[r] = tlen; sh.ring_meta[r] = meta;                                 \
+      // ---- tokens of this lane through the ring (TOK_WIN at a time), one pass per token kind so that the lanes of a pass
+      // run the same code: slot = rank of the token in text order, separators = commas / colons since the previous token
+      const uint32_t cntT = tpw::popc(T);
+      const uint32_t incl = tpw::scan_incl(cntT);
+      const uint32_t lane_off = incl - cntT, total = tpw::shfl(incl, 31);
+      uint32_t other_nx = tpw::shfl_down(other, 1);       // the next lane's scalar bytes: a run may continue there
+      if (l == 31) other_nx = 0xFFFFFFFFu;                // unknown: treated as "continues" -> RM_OPENEND
+      if (done >= total) break;                          // no (more) tokens in this step
+      {
+        const uint32_t win = total - done > TOK_WIN ? TOK_WIN : total - done;
+        const uint32_t lo = done > lane_off ? done - lane_off : 0u, hi = done + win > lane_off ? done + win - lane_off : 0u;   // ranks [lo, hi) of this lane
+  #define TP_TOKEN_PROLOGUE(MASK)                                                                               \
+        for (uint32_t tm = (MASK); tm;) {                                                                       \
+          const uint32_t j = tpw::ffs(tm) - 1;                                                                  \
+          tm &= tm - 1;                                                                                         \
+          const uint32_t below = bits_below(j), rank = tpw::popc(T & below);                                    \
+          if (rank < lo || rank >= hi) continue;                                                                \
+          const uint32_t pt = T & below;                                                                        \
+          uint32_t between = below, nc = sep_in & 0xFFFFu, nk = sep_in >> 16;                                   \
+          if (pt) { between = below & ~bits_below(32 - tpw::clz(pt)); nc = 0; nk = 0; }                         \
+          nc = sat3(nc + tpw::popc(comma_out & between));                                                       \
+          nk = sat3(nk + tpw::popc(colon_out & between));                                                       \
+          uint32_t meta = (nc << RM_NCOMMA_SH) | (nk << RM_NCOLON_SH), tpos = v + j - lead, tlen = 0;           \
+          const uint32_t r = (head + rcount + (lane_off + rank - done)) & (RING - 1);
+  #define TP_TOKEN_EPILOGUE                                                                                     \
+          sh.ring_pos[r] = tpos; sh.ring_len[r] = tlen; rmeta[r] = meta;                                        \
+        }
+        TP_TOKEN_PROLOGUE(brackets)
+          meta |= ((M.ob >> j) & 1u) ? (((M.curly >> j) & 1u) ? K_OPEN_OBJ : K_OPEN_ARR) : (((M.curly >> j) & 1u) ? K_CLOSE_OBJ : K_CLOSE_ARR);
+        TP_TOKEN_EPILOGUE
+        TP_TOKEN_PROLOGUE(closeq)
+          const uint32_t qb = quotes & below;
+          uint32_t span = below, cls = so_cls, op = so_pos;
+          if (qb) { const uint32_t ob = 31 - tpw::clz(qb); op = v + ob; span = below & ~bits_below(ob + 1); cls = 0; }
+          tpos = op + 1 - lead; tlen = (v + j) - op - 1;
+          meta |= K_STR;
+          if ((cls & 1u) | (m_special & span)) meta |= RM_SPECIAL;
+          if ((cls & 2u) | (m_nonkey & span)) meta |= RM_NONKEY;
+          if ((cls & 4u) | (m_hi & span)) meta |= RM_HI;
+          if ((cls & 8u) | (m_bs & span)) meta |= RM_BS;
+        TP_TOKEN_EPILOGUE
+        TP_TOKEN_PROLOGUE(starts)
+          meta |= K_NUM;
+          const uint32_t e = ~other & ~bits_below(j + 1);          // first byte after the run, within the lane
+          if (e) { tlen = tpw::ffs(e) - 1 - j; if (!(range_mask(j, j + tlen) & ~M.digit)) meta |= RM_ALLDIGIT; }
+          else if (~other_nx) tlen = 32 - j + tpw::ffs(~other_nx) - 1;   // ends in the next lane
+          else { tlen = 32 - j; meta |= RM_OPENEND; }
+        TP_TOKEN_EPILOGUE
+  #undef TP_TOKEN_PROLOGUE
+  #undef TP_TOKEN_EPILOGUE
+        rcount += win;
+        tpw::sync();
+        while (rcount >= 33 && !st.status) {
+          const uint32_t la = (rmeta[(head + 32) & (RING - 1)] >> RM_NCOLON_SH) & 3u;
+          tok_batch(s, n, toks, tok_cap, sh, st, head, 32, la, stage, wlo);
+          head += 32; rcount -= 32;
+        }
+        tpw::sync();
       }
-      TP_TOKEN_PROLOGUE(brackets)
-        meta |= ((M.ob >> j) & 1u) ? (((M.curly >> j) & 1u) ? K_OPEN_OBJ : K_OPEN_ARR) : (((M.curly >> j) & 1u) ? K_CLOSE_OBJ : K_CLOSE_ARR);
-      TP_TOKEN_EPILOGUE
-      TP_TOKEN_PROLOGUE(closeq)
-        const uint32_t qb = quotes & below;
-        uint32_t span = below, cls = so_cls, op = so_pos;
-        if (qb) { const uint32_t ob = 31 - tpw::clz(qb); op = v + ob; span = below & ~bits_below(ob + 1); cls = 0; }
-        tpos = op + 1 - lead; tlen = (v + j) - op - 1;
-        meta |= K_STR;
-        if ((cls & 1u) | (m_special & span)) meta |= RM_SPECIAL;
-        if ((cls & 2u) | (m_nonkey & span)) meta |= RM_NONKEY;
-        if ((cls & 4u) | (m_hi & span)) meta |= RM_HI;
-        if ((cls & 8u) | (m_bs & span)) meta |= RM_BS;
-      TP_TOKEN_EPILOGUE
-      TP_TOKEN_PROLOGUE(starts)
-        meta |= K_NUM;
-        const uint32_t e = ~other & ~bits_below(j + 1);          // first byte after the run, within the lane
-        if (e) { tlen = tpw::ffs(e) - 1 - j; if (!(range_mask(j, j + tlen) & ~M.digit)) meta |= RM_ALLDIGIT; }
-        else if (~other_nx) tlen = 32 - j + tpw::ffs(~other_nx) - 1;   // ends in the next lane
-        else { tlen = 32 - j; meta |= RM_OPENEND; }
-      TP_TOKEN_EPILOGUE
-#undef TP_TOKEN_PROLOGUE
-#undef TP_TOKEN_EPILOGUE
-      rcount += win;
-      tpw::sync();
-      while (rcount >= 33 && !st.status) {
-        const uint32_t la = (sh.ring_meta[(head + 32) & (RING - 1)] >> RM_NCOLON_SH) & 3u;
-        tok_batch(s, n, toks, tok_cap, sh, st, head, 32, la, stage, wlo);
-        head += 32; rcount -= 32;
-      }
-      tpw::sync();
+      if (st.status || done + TOK_WIN >= total) break;
     }
     if (st.status) break;
   }
   if (!st.status) {
     const uint32_t steps = (vend + 1023) / 1024;
     const uint32_t wlo = (steps - 1) * 1024 - 1024 - lead;
-    if (c_instr || (c_sep & 0xFFFFu) || (c_sep >> 16)) st.status = TS_NOT_JSON;     // unterminated string / separators after the last token
+    if ((c_bits & 1u) || (c_sep & 0xFFFFu) || (c_sep >> 16)) st.status = TS_NOT_JSON;     // unterminated string / separators after the last token
     while (rcount && !st.status) {
       const uint32_t m = rcount > 32 ? 32u : rcount;
-      const uint32_t la = rcount > 32 ? ((sh.ring_meta[(head + 32) & (RING - 1)] >> RM_NCOLON_SH) & 3u) : 0u;
+      const uint32_t la = rcount > 32 ? ((rmeta[(head + 32) & (RING - 1)] >> RM_NCOLON_SH) & 3u) : 0u;
       tok_batch(s, n, toks, tok_cap, sh, st, head, m, la, stage, wlo);
       head += m; rcount -= m;
     }
@@ -982,13 +1012,15 @@ TP_FN uint32_t an_batch(const uint8_t* s, GTok* toks, uint32_t tok_cap, Shared& 
 
 // Table mode: token i opens a row of the array on top of the stack whose first row (rn members, primitives only) closed.
 // Lane r checks row r against the first row's token pattern; returns the number of leading rows that conform (each of
-// S = 2 + 2 rn tokens) after patching their openers and counting them as children.
-TP_FN uint32_t an_rows(const uint8_t* s, GTok* toks, uint32_t ntok, Shared& sh, uint8_t* stage, AnState& st, uint32_t i) {
+// S = 2 + 2 rn tokens) after patching their openers and counting them as children.  *staged_only: every row the round took
+// conforms, and the round was only cut short because the rows behind them did not fit the staging buffer.
+TP_FN uint32_t an_rows(const uint8_t* s, GTok* toks, uint32_t ntok, Shared& sh, uint8_t* stage, AnState& st, uint32_t i, bool* staged_only) {
   const uint32_t l = tpw::lane();
   const uint32_t top = st.sp - 1;
   const uint32_t rn = sh.row0_n[top], r0 = sh.row0_idx[top] - 1, S = 2 + 2 * rn;
   const uint32_t avail = (ntok - i) / S;
   uint32_t R = avail > 32 ? 32u : avail;
+  const uint32_t R0 = R;
   const uint32_t t0 = i + l * S;
   // source bytes of the candidate rows -> staging buffer (as many leading rows as fit)
   const uint32_t a0 = toks[i].pos;
@@ -1027,6 +1059,7 @@ TP_FN uint32_t an_rows(const uint8_t* s, GTok* toks, uint32_t ntok, Shared& sh, 
     tpw::sync();
     st.last_was_key = 0;
   }
+  *staged_only = ngood == R && R < R0;
   return ngood;
 }
 
@@ -1038,9 +1071,10 @@ TP_FN int analyze(const uint8_t* s, GTok* toks, uint32_t ntok, uint32_t tok_cap,
   while (i < ntok && !st.status) {
     if (!force && st.sp > 0 && table_candidate(sh, st.sp - 1) && gt_kind(toks[i].w) == K_OPEN_OBJ) {
       const uint32_t S = 2 + 2 * sh.row0_n[st.sp - 1];
-      const uint32_t g = an_rows(s, toks, ntok, sh, stage, st, i);
+      bool staged_only;
+      const uint32_t g = an_rows(s, toks, ntok, sh, stage, st, i, &staged_only);
       i += g * S;
-      if (g < 32) force = true;                       // the next row (if it is one) does not conform: generic walk
+      if (g < 32 && !staged_only) force = true;       // the next row (if it is one) does not conform: generic walk
       continue;
     }
     const uint32_t m = ntok - i > 32 ? 32u : ntok - i;
@@ -1333,14 +1367,14 @@ TP_FN void em_rows(const uint8_t* s, const GTok* toks, uint8_t* out, uint32_t ou
     const bool staged_out = Rf && total <= ROW_OUT && !st.over;
     if (act) {
       Emit em;
-      if (staged_out) { em.out = stage + ROW_SRC - st.ocur; em.cap = st.ocur + ROW_OUT; }
+      if (staged_out) { em.out = sh.row_out() - st.ocur; em.cap = st.ocur + ROW_OUT; }
       else { em.out = out; em.cap = out_cap; }
       em.o = off;
       em.put('\n');
       em.spaces(pre);
       for (uint32_t k = 0; k < rn; ++k) { if (k) em.put(','); cell_put(em, sb, toks[t0 + 2 + 2 * k]); }
     }
-    if (staged_out) { tpw::sync(); stage_flush(out, st.ocur, stage + ROW_SRC, total); }
+    if (staged_out) { tpw::sync(); stage_flush(out, st.ocur, sh.row_out(), total); }
     st.ocur += total;
     rb += R;
   }
