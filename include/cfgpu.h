@@ -26,7 +26,7 @@
  *          what `orjson.loads` (toon_encoder.py:281), `serde_json::from_slice` (lib.rs:353) and the
  *          string walk `_iter_strings` (harmful_content_detector.py:110-139) each recompute per payload
  *
- *   cf_run_batch / cf_chain
+ *   cf_run_batch / cf_chain / cf_run_enqueue + cf_run_finish
  *       -> the whole per-request plugin chain over one uploaded batch (mcpgateway/services/tool_service.py:5866-5872)
  *
  * Environment (read once per process):
@@ -99,7 +99,8 @@ int cf_builder_compile_host(cf_builder* b, cf_compile_stats* out);
  * stream's work: calls on ONE cf_ctx must be serialised by the caller (the Python binding holds a lock per context; a gateway
  * worker has one context and one launching thread).  Different cf_ctx objects — one per worker process or per GPU — are
  * independent.  A compiled cf_prog is immutable and may be used by any call of the ctx that compiled it; a cf_batch holds ONE
- * upload at a time.  The asynchronous entry points (cf_scan, cf_toon, cf_chain) only enqueue on the given stream and return. */
+ * upload at a time.  The asynchronous entry points (cf_scan, cf_toon, cf_chain, cf_run_enqueue) only enqueue on the given stream and
+ * return. */
 int cf_init(int device_ordinal, cf_ctx** out);
 void cf_shutdown(cf_ctx* ctx);
 const char* cf_last_error(cf_ctx* ctx);
@@ -242,6 +243,44 @@ int cf_copy_to_host(cf_ctx* ctx, void* host_dst, const void* device_src, uint64_
 int cf_chain(cf_ctx* ctx, cf_prog* prog, cf_batch* b, uint32_t stage_mask, uint32_t toon_flags, uint64_t* d_bitmaps, const uint8_t* d_unit_stages,
              uint8_t* d_out, uint32_t* d_out_len, int32_t* d_status, void* cuda_stream);
 
+/* ---------------- the fused chain on the caller's stream: cf_run_enqueue / cf_run_finish ----------------
+ * cf_run_batch's SCAN, SUB and TOON stages without a host round trip between launch and completion: the dirty-unit selection, the
+ * substitution's scratch bounds and arena allocation, the verdict records, the output offsets and the gather are decided on the
+ * device.  cf_run_batch itself (without CF_STAGE_MASK) is an upload, one enqueue and one finish on a run the context owns.
+ *
+ * A cf_run owns every piece of per-call device state (scan queue, TOON scratch and unit order, the dirty-unit list, the substitution
+ * descriptors and arena, per-unit gather sources, a status block, a completion event and a side stream), so runs created on one
+ * ctx can be in flight at once on different streams.  Memory of a run: 8 x max_stream_bytes of TOON scratch, max_stream_bytes of
+ * TOON output, about 170 bytes per unit, 8 MiB of scan queue and the arena.  (The run cf_run_batch uses borrows the context's TOON
+ * workspace instead, the one cf_toon and cf_chain use, so a context holds one.)
+ *
+ * cf_run_enqueue: the batch must be resident (cf_batch_upload on the same stream, or ordered before it).  d_verdicts (n_units
+ * records), d_out_offsets (n_units + 1), d_out (out_cap bytes), d_bitmaps_full (n_units * W words; required with SCAN or SUB) and
+ * d_unit_stages (may be NULL) are caller-owned DEVICE memory (torch tensors work).  Stages: CF_STAGE_SCAN, CF_STAGE_SUB (implies
+ * SCAN), CF_STAGE_TOON; CF_STAGE_MASK is CF_E_BADARG (masking keeps cf_run_batch).  Results are cf_run_batch's, unit for unit.
+ * Between its first launch and its return the call neither synchronises, allocates nor reads device memory on the host, so it
+ * can be captured in a CUDA graph.  Warm the run up with one enqueue + finish first, so that the arena has its size; a replay that
+ * needs more defers the units that do not fit, and the graph stays valid: once an enqueue of a run was captured, arenas the run
+ * outgrows are kept until cf_run_free.  The batch, the program and every buffer passed in must stay untouched until cf_run_finish
+ * returns.  Every check that can fail is made before the first launch, so an error return leaves nothing queued.
+ *
+ * Deferred units: a dirty unit whose two scratch buffers (first-pass bound min(worst, 64 L + 64 KiB) each, as cf_sub_host) do not fit
+ * the arena that is left, or whose rewrite outgrows that bound, gets no output in the enqueue.  cf_run_finish completes it with the
+ * synchronous substitution (which regrows its room and reports CF_E_TOO_LARGE), patches its record and redoes offsets and gather.
+ *
+ * cf_run_finish: waits for the run's last enqueue (or a graph replay of it) and reads its status through the run's own non-blocking
+ * stream (it waits for nothing else the caller has queued).  Returns CF_OK; CF_E_CAPACITY only when the gathered texts need
+ * *needed > out_cap bytes (verdicts and out_offsets are valid, d_out is untouched); CF_E_TOO_LARGE when a deferred unit's substitution
+ * exceeds one of its limits (the worst-case bound, a unit beyond 4 GB, scratch beyond 8 GiB: cf_last_error says which); or another
+ * error.  *needed (may be NULL) = bytes of all gathered texts, 0 on any error other than CF_E_CAPACITY.  It grows the arena to what
+ * the call asked for, for the next call. */
+typedef struct cf_run cf_run;
+int cf_run_create(cf_ctx* ctx, uint32_t max_units, uint64_t max_stream_bytes, uint64_t sub_arena_bytes, cf_run** out);
+void cf_run_free(cf_run* run);
+int cf_run_enqueue(cf_ctx* ctx, cf_prog* prog, cf_batch* b, cf_run* run, uint32_t stage_mask, const uint8_t* d_unit_stages, uint32_t toon_flags,
+                   cf_verdict* d_verdicts, uint64_t* d_bitmaps_full, uint64_t* d_out_offsets, uint8_t* d_out, uint64_t out_cap, void* cuda_stream);
+int cf_run_finish(cf_ctx* ctx, cf_run* run, uint64_t* needed);
+
 /* number of kernels launched by this ctx so far (for bench.py's gpu_launches) */
 uint64_t cf_kernel_launches(const cf_ctx* ctx);
 
@@ -252,7 +291,8 @@ int cf_profile_collect(cf_ctx* ctx, double* total_ms, uint32_t* n_launches);
 /* same, one duration per recorded launch, in launch order (cf_scan and the TOON stage record one pair each); resets the list */
 int cf_profile_collect_each(cf_ctx* ctx, double* ms, uint32_t cap, uint32_t* n_launches);
 
-/* last scan's device-side counters: [0]=prefilter candidates, [1]=DFA verify steps */
+/* device-side counters of the last cf_scan / cf_scan_host / CF_STAGE_MASK cf_run_batch scan: [0]=prefilter candidates, [1]=DFA verify
+ * steps.  cf_run_enqueue (and cf_run_batch without CF_STAGE_MASK, which runs through it) counts on its run's own pair. */
 int cf_scan_counters(cf_ctx* ctx, uint64_t out[2]);
 
 #ifdef __cplusplus

@@ -40,9 +40,7 @@ struct cf_ctx {
   size_t h_stage_bytes = 0;
   const uint8_t* run_out = nullptr;   // device buffer of the last CF_RUN_OUTPUTS_RESIDENT call
   uint64_t run_out_bytes = 0;
-  // cf_run_batch: the substitution runs on `side` (non-blocking, highest priority) beside the TOON kernel on the legacy stream
-  cudaStream_t side = nullptr;
-  cudaEvent_t ev_scan = nullptr, ev_toon = nullptr, ev_sub = nullptr;
+  cf_run* run = nullptr;              // cf_run_batch's run (legacy stream), grown with the batches
   // optional per-launch timing of the dominant kernel (bench.py roofline): event pairs
   std::vector<cudaEvent_t> prof_ev;
   uint32_t prof_used = 0;
@@ -56,6 +54,9 @@ struct cf_ctx {
   uint32_t tile() const { return scan_warps * 32 * scan_lane_bytes; }
   uint32_t box_rows() const { uint32_t rows = tile() / 128, nbox = (rows + 255) / 256; return rows / nbox; }
 };
+
+// the figures of an ordered rule that bound its output's growth (cf_sub_device's `worst`)
+struct RuleGrowth { uint32_t minlen, repl_len, n_parts, nrefs, lit_len; };
 
 struct DevDfa {
   cf::DfaTables t;
@@ -83,6 +84,10 @@ struct cf_prog {
     uint32_t ninst = 0, wpc = 1, nslots = 2, n_parts = 0, nrefs = 0, lit_len = 0;
   };
   std::vector<RuleTmpl> tmpl;             // per ordered rule
+  std::vector<RuleGrowth> growth;         // per ordered rule: the figures of the scratch bound (host and device copy; cf_run_enqueue
+  RuleGrowth* d_growth = nullptr;         // computes the bound on the device)
+  uint64_t* d_rule_mask = nullptr;        // W words: the bits of the CF_PAT_ORDERED patterns
+  uint32_t pike_words = 0;                // Pike-VM scratch words per unit of the largest template rule (0: no template rule)
   std::vector<uint64_t> h_offsets;        // host copy of the last batch's offsets (cf_sub_host sizing)
   const void* h_offsets_owner = nullptr;
   uint64_t h_offsets_gen = 0;
@@ -125,6 +130,75 @@ int cf_stage_reserve(cf_ctx* ctx, size_t need);
 size_t cf_sub_stage_bytes(uint32_t n_sel);
 int cf_sub_device(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint64_t* h_offsets, const uint32_t* units, uint32_t n_sel, cudaStream_t st,
                   uint8_t* h_stage, const uint64_t** rec);
+
+static const uint64_t SUB_OVERFLOW = ~1ull;     // record[0] of a unit whose output outgrew its scratch bound (record[1] = the rule)
+
+// ---- cf_run (include/cfgpu.h): the state of one asynchronous chain
+// device status block of a run, zeroed at the start of every enqueue
+struct RunStatus {
+  int32_t err;            // CF_E_CAPACITY when the gathered texts exceed out_cap (the gather is skipped)
+  uint32_t n_sel;         // dirty units the enqueue rewrites (selection list length)
+  uint32_t n_deferred;    // dirty units left to cf_run_finish
+  uint32_t pad;
+  uint64_t needed;        // bytes of all gathered texts
+  uint64_t arena_used;    // substitution arena bytes the dirty units asked for (fitting or not)
+};
+static const uint32_t RUN_NOT_DIRTY = 0xFFFFFFFFu;    // slot[u]: the unit is not rewritten
+static const uint32_t RUN_DEFER_PENDING = 0xFFFFFFFEu;  // ... dirty, did not fit the arena
+static const uint32_t RUN_DEFER = 0x80000000u;        // ... deferred, RUN_DEFER | index in the deferred list; otherwise the selection index
+
+struct cf_run {
+  cf_ctx* ctx = nullptr;
+  uint32_t max_units = 0;
+  uint64_t max_bytes = 0;
+  std::vector<void*> allocs;
+  cudaStream_t side = nullptr;                          // the substitution, beside TOON
+  cudaEvent_t ev_scan = nullptr, ev_sub = nullptr, ev_done = nullptr;
+  uint64_t* d_queue = nullptr;                          // scan candidate queue and its counters
+  uint64_t* d_qstate = nullptr;
+  uint32_t qphase = 0;
+  void* d_toon_scratch = nullptr;                       // TOON: token / DOM scratch, unit order and its sort
+  uint64_t toon_scratch_bytes = 0;
+  uint32_t* d_toon_order = nullptr;
+  uint8_t* d_toon_sort = nullptr;
+  size_t toon_sort_bytes = 0;
+  uint8_t* d_toon_out = nullptr;                        // TOON texts in the input's layout
+  uint32_t* d_toon_ls = nullptr;                        // TOON lengths [n] | statuses [n]
+  uint32_t* d_slot = nullptr;                           // per unit: RUN_NOT_DIRTY / selection index / RUN_DEFER*
+  uint32_t* d_sel = nullptr;                            // per selection index: unit, scratch offset, bound, record
+  uint64_t *d_soff = nullptr, *d_bound = nullptr, *d_rec = nullptr;
+  uint8_t* d_arena = nullptr;
+  uint64_t arena_bytes = 0;
+  bool ever_captured = false;                           // an enqueue was captured in a CUDA graph: arenas it may use are kept
+  std::vector<void*> retired;                           // ... here, until cf_run_free
+  uint8_t* enq_arena = nullptr;                         // the arena the last enqueue (or the graph replaying it) rewrote into
+  uint32_t* d_deferred = nullptr;                       // deferred units; d_def_rec: their records after cf_run_finish
+  uint64_t* d_def_rec = nullptr;
+  uint64_t* d_src = nullptr;                            // per unit: device address of its produced text
+  uint64_t* d_len = nullptr;                            // per unit: its length, [n] = 0 (scanned into out_offsets)
+  void* d_scan_tmp = nullptr;
+  size_t scan_tmp_bytes = 0;
+  RunStatus* d_status = nullptr;
+  RunStatus* h_status = nullptr;                        // pinned
+  // the last enqueue
+  cf_prog* prog = nullptr;
+  cf_batch* batch = nullptr;
+  cudaStream_t st = nullptr;
+  uint32_t stage_mask = 0;
+  const uint8_t* d_unit_stages = nullptr;
+  cf_verdict* d_verdicts = nullptr;
+  const uint64_t* d_bitmaps = nullptr;
+  uint32_t W = 1;
+  bool sub = false;                                     // the substitution ran (d_slot is valid)
+  uint64_t* d_out_offsets = nullptr;
+  uint8_t* d_out = nullptr;
+  uint64_t out_cap = 0;
+};
+
+// the scan of cf_scan on a given candidate queue / counter pair (cfgpu.cu)
+int cf_scan_launch(cf_ctx* ctx, cf_prog* p, cf_batch* b, uint64_t* d_bitmaps, cudaStream_t st, uint64_t* queue, uint64_t* qstate, uint32_t* qphase);
+// cf_run_enqueue's substitution on `st` (cfgpu.cu): dirty-unit selection, bounds and arena allocation, then the sub_kernel launches
+int cf_sub_enqueue(cf_ctx* ctx, cf_prog* p, cf_batch* b, cf_run* run, const uint64_t* d_bitmaps, const uint8_t* d_unit_stages, cudaStream_t st);
 
 // sequential JSON kernels (cfjson_seq.cu)
 namespace cfj { struct JNode; }

@@ -581,7 +581,6 @@ static const ScanVariant* scan_variant(uint32_t warps, uint32_t lane_bytes, uint
 static const uint32_t SUB_LAUNCH_RULES = 32;    // rules per sub_kernel launch; longer programs continue in further launches
 static const uint32_t SUB_WIN = 512;            // start positions examined per warp iteration
 static const uint32_t SUB_WARPS = 4;
-static const uint64_t SUB_OVERFLOW = ~1ull;     // rec[0] of a unit whose output outgrew its scratch bound (rec[1] = the rule)
 
 struct SubRule {
   cf::DfaTables dfa;
@@ -603,9 +602,11 @@ struct SubParams {
   const uint64_t* bound;
   uint8_t* scratch;
   uint64_t* rec;              // per selected unit: [0] = text offset in scratch (~0: unchanged, SUB_OVERFLOW), [1] = length
-  uint32_t* pike;             // per selected unit: pike_words of Pike-VM scratch (rules with group references only)
+  uint32_t* pike;             // per selected unit: pike_words of Pike-VM scratch (rules with group references only); NULL with
+                              // pike_words != 0: in the unit's scratch area, behind its two buffers
   uint64_t pike_words;
   uint32_t n_sel;
+  const uint32_t* n_dev;      // not NULL: the number of selected units is on the device (the grid covers n_sel)
   uint32_t n_rules;
   uint32_t first_rule;        // program index of rules[0]
   uint32_t resume;            // 0: start from the stream; 1: continue from `rec` (a previous launch's rules)
@@ -646,10 +647,11 @@ __global__ void __launch_bounds__(SUB_WARPS * 32) sub_kernel(const __grid_consta
   __shared__ uint32_t caps_all[SUB_WARPS][64];
   const uint32_t lane = threadIdx.x & 31, wic = threadIdx.x >> 5;
   const uint32_t w = blockIdx.x * SUB_WARPS + wic;
-  if (w >= P.n_sel) return;
+  if (w >= (P.n_dev ? *P.n_dev : P.n_sel)) return;
   uint32_t* mlen = mlen_s[wic];
   uint32_t* caps_s = caps_all[wic];
-  uint32_t* pike = P.pike ? P.pike + (uint64_t)w * P.pike_words : nullptr;
+  uint32_t* pike = nullptr;
+  if (P.pike_words) pike = P.pike ? P.pike + (uint64_t)w * P.pike_words : reinterpret_cast<uint32_t*>(P.scratch + P.soff[w] + 2 * P.bound[w]);
   const uint32_t u = P.sel[w];
   const uint8_t* src = P.stream + P.offsets[u];
   uint64_t len = P.offsets[u + 1] - P.offsets[u] - 1;
@@ -778,6 +780,65 @@ __global__ void __launch_bounds__(SUB_WARPS * 32) sub_kernel(const __grid_consta
   }
 }
 
+// Scratch bound of a unit of `len` bytes: worst = its worst-case growth through all rules.  A rule with matches of >= ml characters
+// (so >= ml bytes) turns L bytes into at most L * ceil(repl / ml); a rule that can match "" has at most L + 1 empty and L non-empty
+// matches; a template emits its literals and each referenced group (at most the match itself) per match.  Over a long program that
+// product is far above what any text needs (a -> bb, bb -> c, ... doubles it at every other rule), so the first pass gives a unit at
+// most 64 L + 64 KiB.  Host (cf_sub_device) and device (sub_select_kernel) share the formula.
+__host__ __device__ inline double sub_worst(uint64_t len, const RuleGrowth* g, uint32_t nr) {
+  double bd = (double)len;
+  for (uint32_t r = 0; r < nr; ++r) {
+    const uint32_t ml = g[r].minlen;
+    if (g[r].n_parts) {
+      const double nmatch = ml ? bd / ml + 1.0 : 2.0 * bd + 1.0;
+      bd = bd * (1.0 + g[r].nrefs) + nmatch * (double)g[r].lit_len;
+    } else if (ml == 0) bd += (2.0 * bd + 1.0) * (double)g[r].repl_len;
+    else { const double f = (double)((g[r].repl_len + ml - 1) / ml); if (f > 1.0) bd *= f; }
+  }
+  return bd + 16.0;
+}
+__host__ __device__ inline uint64_t sub_round16(double x) { return ((uint64_t)x + 15) & ~15ull; }
+__host__ __device__ inline uint64_t sub_first_bound(uint64_t len, double worst) {
+  const double cap = 64.0 * (double)len + 65536.0;
+  return sub_round16(worst < cap ? worst : cap);
+}
+
+// cf_run_enqueue: the dirty units (a CF_PAT_ORDERED bit set, SUB allowed by the unit's stages), their first-pass bounds, and their two
+// scratch buffers (+ Pike-VM words) from the run's arena by an atomic cursor.  The units that fit are compacted with a warp ballot
+// into sel / soff / bound (slot[u] = selection index); the others are deferred to cf_run_finish.  The cursor's final value is what
+// the call needed: every dirty unit adds to it, fitting or not.
+__global__ void __launch_bounds__(256) sub_select_kernel(const uint64_t* __restrict__ bm, uint32_t W, const uint64_t* __restrict__ rule_mask,
+                                                         const uint8_t* __restrict__ unit_stages, const uint64_t* __restrict__ offsets, uint32_t n,
+                                                         const RuleGrowth* __restrict__ g, uint32_t nr, uint64_t pike_bytes, uint64_t arena_bytes,
+                                                         RunStatus* st, uint32_t* __restrict__ slot, uint32_t* __restrict__ sel,
+                                                         uint64_t* __restrict__ soff, uint64_t* __restrict__ bound) {
+  const uint32_t u = blockIdx.x * blockDim.x + threadIdx.x, lane = threadIdx.x & 31;
+  bool dirty = false, fit = false;
+  uint64_t off = 0, bd = 0;
+  if (u < n && (!unit_stages || (unit_stages[u] & CF_STAGE_SUB)))
+    for (uint32_t w = 0; w < W; ++w)
+      if (bm[(uint64_t)u * W + w] & rule_mask[w]) { dirty = true; break; }
+  if (dirty) {
+    const uint64_t len = offsets[u + 1] - offsets[u] - 1;
+    bd = sub_first_bound(len, sub_worst(len, g, nr));
+    const uint64_t need = 2 * bd + pike_bytes;
+    off = atomicAdd(reinterpret_cast<unsigned long long*>(&st->arena_used), (unsigned long long)need);
+    fit = off + need <= arena_bytes;
+  }
+  const uint32_t m = __ballot_sync(0xFFFFFFFFu, fit);
+  uint32_t base = 0;
+  if (lane == 0 && m) base = atomicAdd(&st->n_sel, (uint32_t)__popc(m));
+  base = __shfl_sync(0xFFFFFFFFu, base, 0);
+  if (u >= n) return;
+  if (fit) {
+    const uint32_t w = base + __popc(m & ((1u << lane) - 1u));
+    sel[w] = u;
+    soff[w] = off;
+    bound[w] = bd;
+    slot[u] = w;
+  } else slot[u] = dirty ? RUN_DEFER_PENDING : RUN_NOT_DIRTY;
+}
+
 __global__ void sub_compact_kernel(const uint8_t* __restrict__ stream, const uint64_t* __restrict__ offsets,
                                    const uint32_t* __restrict__ sel, const uint8_t* __restrict__ scratch,
                                    const uint64_t* __restrict__ rec, const uint64_t* __restrict__ out_off,
@@ -832,6 +893,56 @@ static size_t sub_desc_bytes(uint32_t n) { return ((size_t)n * 20 + 15) & ~(size
 static const uint32_t* sub_desc_sel(const cf_ctx* ctx, uint32_t n) { return (const uint32_t*)((const uint64_t*)ctx->tmp[9].p + 2 * (size_t)n); }
 size_t cf_sub_stage_bytes(uint32_t n_sel) { return sub_desc_bytes(n_sel) + (size_t)n_sel * 16; }
 
+// the sub_kernel launches of one pass: SUB_LAUNCH_RULES rules per launch; each further launch continues every unit from the record
+// the previous one left
+static int sub_launch_rules(cf_ctx* ctx, const cf_prog* p, SubParams& SP, cudaStream_t st) {
+  const uint32_t nr = (uint32_t)p->ordered.size();
+  for (uint32_t r0 = 0; r0 < nr; r0 += SUB_LAUNCH_RULES) {
+    SP.first_rule = r0;
+    SP.resume = r0 > 0;
+    SP.n_rules = std::min(nr - r0, SUB_LAUNCH_RULES);
+    for (uint32_t i = 0; i < SP.n_rules; ++i) {
+      const uint32_t r = r0 + i;
+      SubRule& S = SP.rules[i];
+      S.dfa = p->ordered[r].t;
+      S.E = p->d_ordered_E[r];
+      S.repl = p->d_repl[r];
+      S.repl_len = p->repl_len[r];
+      S.nullable = p->ordered_minlen[r] == 0;
+      const cf_prog::RuleTmpl& T = p->tmpl[r];
+      S.parts = T.d_parts;
+      S.n_parts = T.n_parts;
+      S.nfa.code = T.d_code; S.nfa.setbits = T.d_sets;
+      S.nfa.ninst = T.ninst; S.nfa.start = 0; S.nfa.wpc = T.wpc; S.nfa.nslots = T.nslots;
+    }
+    sub_kernel<<<(SP.n_sel + SUB_WARPS - 1) / SUB_WARPS, SUB_WARPS * 32, 0, st>>>(SP);
+    ctx->launches++;
+    CF_CUDA(ctx, cudaGetLastError());
+  }
+  return CF_OK;
+}
+
+int cf_sub_enqueue(cf_ctx* ctx, cf_prog* p, cf_batch* b, cf_run* run, const uint64_t* d_bitmaps, const uint8_t* d_unit_stages, cudaStream_t st) {
+  const uint32_t n = b->n;
+  const uint64_t pike_bytes = ((uint64_t)p->pike_words * 4 + 15) & ~15ull;
+  sub_select_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_bitmaps, p->W, p->d_rule_mask, d_unit_stages, b->d_offsets, n, p->d_growth,
+                                                     (uint32_t)p->ordered.size(), pike_bytes, run->arena_bytes, run->d_status, run->d_slot,
+                                                     run->d_sel, run->d_soff, run->d_bound);
+  ctx->launches++;
+  CF_CUDA(ctx, cudaGetLastError());
+  // the launches are sized for every unit; warps past the device's count of selected units exit at once
+  SubParams SP;
+  SP.stream = b->d_buf + cf::FRONT_PAD;
+  SP.offsets = b->d_offsets;
+  SP.sel = run->d_sel; SP.soff = run->d_soff; SP.bound = run->d_bound;
+  SP.scratch = run->d_arena;
+  SP.rec = run->d_rec;
+  SP.pike = nullptr; SP.pike_words = p->pike_words;
+  SP.n_sel = n;
+  SP.n_dev = &run->d_status->n_sel;
+  return sub_launch_rules(ctx, p, SP, st);
+}
+
 int cf_sub_device(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint64_t* h_offsets, const uint32_t* units, uint32_t n_sel, cudaStream_t st,
                   uint8_t* h_stage, const uint64_t** rec_out) {
   const uint32_t nr = (uint32_t)p->ordered.size();
@@ -840,30 +951,16 @@ int cf_sub_device(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint64_t* h_offset
   uint64_t* bound = soff + n_sel;
   uint32_t* sel = (uint32_t*)(bound + n_sel);
   uint64_t* rec = (uint64_t*)(h_stage + sub_desc_bytes(n_sel));
-  // Scratch: two buffers of bound[i] bytes per selected unit.  worst[i] = the unit's worst-case growth through all rules: a rule with
-  // matches of >= ml characters (so >= ml bytes) turns L bytes into at most L * ceil(repl / ml); a rule that can match "" has at most
-  // L + 1 empty and L non-empty matches.  Over a long program that product is far above what any text needs (a -> bb, bb -> c, ...
-  // doubles it at every other rule), so the first pass gives a unit at most 64 L + 64 KiB.  The kernel clamps every write to the
-  // unit's bound and reports a unit whose output outgrew it; that unit runs again with 8x the room, up to worst[i].  Outgrowing
-  // worst[i] itself is an internal error (CF_E_TOO_LARGE), never a write into a neighbour's scratch.
+  // Scratch: two buffers of bound[i] bytes per selected unit, first sub_first_bound.  The kernel clamps every write to the unit's bound
+  // and reports a unit whose output outgrew it; that unit runs again with 8x the room, up to worst[i].  Outgrowing worst[i] itself is
+  // an internal error (CF_E_TOO_LARGE), never a write into a neighbour's scratch.
   std::vector<double> worst(n_sel);
-  auto round16 = [](double x) { return ((uint64_t)x + 15) & ~15ull; };
   for (uint32_t i = 0; i < n_sel; ++i) {
     if (units[i] >= b->n) { ctx->err = "unit index out of range"; return CF_E_BADARG; }
     sel[i] = units[i];
     uint64_t len = h_offsets[units[i] + 1] - h_offsets[units[i]] - 1;
-    double bd = (double)len;
-    for (uint32_t r = 0; r < nr; ++r) {
-      const uint32_t ml = p->ordered_minlen[r];
-      const cf_prog::RuleTmpl& T = p->tmpl[r];
-      if (T.n_parts) {             // every match: its literals + each referenced group (at most the match itself)
-        const double nmatch = ml ? bd / ml + 1.0 : 2.0 * bd + 1.0;
-        bd = bd * (1.0 + T.nrefs) + nmatch * (double)T.lit_len;
-      } else if (ml == 0) bd += (2.0 * bd + 1.0) * (double)p->repl_len[r];
-      else { const double g = (double)((p->repl_len[r] + ml - 1) / ml); if (g > 1.0) bd *= g; }
-    }
-    worst[i] = bd + 16.0;
-    bound[i] = round16(std::min(worst[i], 64.0 * (double)len + 65536.0));
+    worst[i] = sub_worst(len, p->growth.data(), nr);
+    bound[i] = sub_first_bound(len, worst[i]);
   }
   int rc;
   // grow-only scratch of the context: no cudaMalloc / cudaFree per call
@@ -875,9 +972,8 @@ int cf_sub_device(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint64_t* h_offset
   SP.soff = d_desc; SP.bound = d_desc + n_sel; SP.sel = sub_desc_sel(ctx, n_sel);
   SP.rec = (uint64_t*)ctx->tmp[12].p;
   SP.n_sel = n_sel;
-  SP.pike = nullptr; SP.pike_words = 0;
-  for (uint32_t r = 0; r < nr; ++r)
-    if (p->tmpl[r].n_parts) { const uint64_t wds = cf::pike_scratch_words(p->tmpl[r].ninst, p->tmpl[r].nslots); if (wds > SP.pike_words) SP.pike_words = wds; }
+  SP.n_dev = nullptr;
+  SP.pike = nullptr; SP.pike_words = p->pike_words;
   if (SP.pike_words) {
     if ((uint64_t)n_sel * SP.pike_words * 4 > (4ull << 30)) { ctx->err = "capture scratch exceeds 4 GiB (too many units for a rule with group references)"; return CF_E_CAPACITY; }
     if ((rc = cf_dev_reserve(ctx, ctx->tmp[15], (size_t)n_sel * SP.pike_words * 4))) return rc;
@@ -891,29 +987,7 @@ int cf_sub_device(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint64_t* h_offset
     if ((rc = cf_dev_reserve(ctx, ctx->tmp[8], total))) return rc;
     SP.scratch = (uint8_t*)ctx->tmp[8].p;
     CF_CUDA(ctx, cudaMemcpyAsync(d_desc, h_stage, sub_desc_bytes(n_sel), cudaMemcpyHostToDevice, st));
-    // SUB_LAUNCH_RULES rules per launch; each further launch continues every unit from the record the previous one left
-    for (uint32_t r0 = 0; r0 < nr; r0 += SUB_LAUNCH_RULES) {
-      SP.first_rule = r0;
-      SP.resume = r0 > 0;
-      SP.n_rules = std::min(nr - r0, SUB_LAUNCH_RULES);
-      for (uint32_t i = 0; i < SP.n_rules; ++i) {
-        const uint32_t r = r0 + i;
-        SubRule& S = SP.rules[i];
-        S.dfa = p->ordered[r].t;
-        S.E = p->d_ordered_E[r];
-        S.repl = p->d_repl[r];
-        S.repl_len = p->repl_len[r];
-        S.nullable = p->ordered_minlen[r] == 0;
-        const cf_prog::RuleTmpl& T = p->tmpl[r];
-        S.parts = T.d_parts;
-        S.n_parts = T.n_parts;
-        S.nfa.code = T.d_code; S.nfa.setbits = T.d_sets;
-        S.nfa.ninst = T.ninst; S.nfa.start = 0; S.nfa.wpc = T.wpc; S.nfa.nslots = T.nslots;
-      }
-      sub_kernel<<<(n_sel + SUB_WARPS - 1) / SUB_WARPS, SUB_WARPS * 32, 0, st>>>(SP);
-      ctx->launches++;
-      CF_CUDA(ctx, cudaGetLastError());
-    }
+    if ((rc = sub_launch_rules(ctx, p, SP, st))) return rc;
     CF_CUDA(ctx, cudaMemcpyAsync(rec, SP.rec, (size_t)n_sel * 16, cudaMemcpyDeviceToHost, st));
     CF_CUDA(ctx, cudaStreamSynchronize(st));
     for (uint32_t i = 0; i < n_sel; ++i) {
@@ -925,7 +999,7 @@ int cf_sub_device(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint64_t* h_offset
         return CF_E_TOO_LARGE;
       }
       if (grown > 4e9) { ctx->err = "substitution rules expand a unit beyond 4 GB"; return CF_E_CAPACITY; }
-      bound[i] = round16(grown);
+      bound[i] = sub_round16(grown);
       again = true;
     }
   }
@@ -951,10 +1025,6 @@ int cf_init(int device_ordinal, cf_ctx** out) {
   CF_CUDA(ctx, cudaMalloc(&ctx->d_qstate, 4 * sizeof(uint64_t)));
   CF_CUDA(ctx, cudaMemset(ctx->d_qstate, 0, 4 * sizeof(uint64_t)));
   CF_CUDA(ctx, cudaMalloc(&ctx->d_queue, (size_t)ctx->qcap * sizeof(uint64_t)));
-  int prio_lo = 0, prio_hi = 0;   // the few substitution blocks take SMs as TOON blocks retire instead of queueing behind all of them
-  CF_CUDA(ctx, cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
-  CF_CUDA(ctx, cudaStreamCreateWithPriority(&ctx->side, cudaStreamNonBlocking, prio_hi));
-  for (cudaEvent_t* e : {&ctx->ev_scan, &ctx->ev_toon, &ctx->ev_sub}) CF_CUDA(ctx, cudaEventCreateWithFlags(e, cudaEventDisableTiming));
   if (const char* e = getenv("CF_SCAN_WARPS")) ctx->scan_warps = (uint32_t)atoi(e);
   if (const char* e = getenv("CF_SCAN_ACC")) ctx->scan_acc = (uint32_t)atoi(e);
   if (const char* e = getenv("CF_SCAN_LB")) ctx->scan_lane_bytes = (uint32_t)atoi(e);
@@ -978,8 +1048,7 @@ void cf_shutdown(cf_ctx* ctx) {
   cudaFree(ctx->d_tok.p); cudaFree(ctx->d_ntok.p);
   cudaFree(ctx->toon_order.p); cudaFree(ctx->toon_sort.p);
   if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
-  if (ctx->side) cudaStreamDestroy(ctx->side);
-  for (cudaEvent_t e : {ctx->ev_scan, ctx->ev_toon, ctx->ev_sub}) if (e) cudaEventDestroy(e);
+  cf_run_free(ctx->run);
   delete ctx;
 }
 
@@ -1044,7 +1113,17 @@ int cf_compile(cf_ctx* ctx, cf_builder* b, cf_prog** out) {
       CF_CUDA(ctx, cudaMemcpy(T.d_parts, b->tmpl[i].data(), b->tmpl[i].size() * 4, cudaMemcpyHostToDevice));
     }
     p->tmpl.push_back(T);
+    p->growth.push_back({p->ordered_minlen.back(), (uint32_t)rl, T.n_parts, T.nrefs, T.lit_len});
+    if (T.n_parts) p->pike_words = std::max(p->pike_words, (uint32_t)cf::pike_scratch_words(T.ninst, T.nslots));
     ++oi;
+  }
+  std::vector<uint64_t> rule_mask(p->W, 0);
+  for (int pi : p->ordered_pat) rule_mask[(size_t)pi / 64] |= 1ull << (pi % 64);
+  CF_CUDA(ctx, cudaMalloc(&p->d_rule_mask, p->W * 8));
+  CF_CUDA(ctx, cudaMemcpy(p->d_rule_mask, rule_mask.data(), p->W * 8, cudaMemcpyHostToDevice));
+  if (!p->growth.empty()) {
+    CF_CUDA(ctx, cudaMalloc(&p->d_growth, p->growth.size() * sizeof(RuleGrowth)));
+    CF_CUDA(ctx, cudaMemcpy(p->d_growth, p->growth.data(), p->growth.size() * sizeof(RuleGrowth), cudaMemcpyHostToDevice));
   }
   return CF_OK;
 }
@@ -1059,6 +1138,8 @@ void cf_free_prog(cf_prog* p) {
   for (auto& t : p->tmpl) { cudaFree(t.d_code); cudaFree(t.d_sets); cudaFree(t.d_parts); }
   cudaFree(p->d_E);
   cudaFree(p->d_always);
+  cudaFree(p->d_rule_mask);
+  cudaFree(p->d_growth);
   delete p;
 }
 
@@ -1158,7 +1239,11 @@ int cf_batch_upload(cf_ctx* ctx, cf_batch* b, const uint8_t* stream, uint64_t st
 
 int cf_scan(cf_ctx* ctx, cf_prog* p, cf_batch* b, uint64_t* d_bitmaps, void* cuda_stream) {
   if (!ctx || !p || !b || !d_bitmaps || !b->n) return CF_E_BADARG;
-  cudaStream_t st = (cudaStream_t)cuda_stream;
+  return cf_scan_launch(ctx, p, b, d_bitmaps, (cudaStream_t)cuda_stream, ctx->d_queue, ctx->d_qstate, &ctx->qphase);
+}
+}  // extern "C"
+
+int cf_scan_launch(cf_ctx* ctx, cf_prog* p, cf_batch* b, uint64_t* d_bitmaps, cudaStream_t st, uint64_t* queue, uint64_t* qstate, uint32_t* qphase) {
   const uint32_t tile = ctx->tile();
   const uint64_t ntiles = ntiles_for(b->nbytes, tile);
   const uint64_t total = (uint64_t)b->n * p->W;
@@ -1180,10 +1265,10 @@ int cf_scan(cf_ctx* ctx, cf_prog* p, cf_batch* b, uint64_t* d_bitmaps, void* cud
   P.E = p->d_E;
   P.dfa = p->search.t;
   P.bitmaps = (unsigned long long*)d_bitmaps;
-  P.queue = (unsigned long long*)ctx->d_queue;
-  P.qstate = (unsigned long long*)ctx->d_qstate + 2 * ctx->qphase;
-  P.qstate_next = (unsigned long long*)ctx->d_qstate + 2 * (ctx->qphase ^ 1);
-  ctx->qphase ^= 1;
+  P.queue = (unsigned long long*)queue;
+  P.qstate = (unsigned long long*)qstate + 2 * *qphase;
+  P.qstate_next = (unsigned long long*)qstate + 2 * (*qphase ^ 1);
+  *qphase ^= 1;
   P.qcap_cta = ctx->qcap / (uint32_t)ctx->sm_count;
   P.dfa_bytes = p->search.stage_bytes < (1u << 30) ? (uint32_t)p->search.stage_bytes : 0;
   P.dfa_trans_bytes = (uint32_t)p->search.trans_bytes;
@@ -1203,7 +1288,7 @@ int cf_scan(cf_ctx* ctx, cf_prog* p, cf_batch* b, uint64_t* d_bitmaps, void* cud
   return CF_OK;
 }
 
-
+extern "C" {
 int cf_scan_host(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint8_t* stream, uint64_t stream_bytes,
                  const uint64_t* offsets, uint32_t n_units, uint64_t* h_bitmaps) {
   if (!h_bitmaps) return CF_E_BADARG;

@@ -5,7 +5,11 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
+#include <type_traits>
+
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 #include <nvtx3/nvToolsExt.h>
 
 #include "cf_internal.h"
@@ -259,11 +263,87 @@ int cf_json_index_host(cf_ctx* ctx, cf_batch* b, uint32_t flags, const uint8_t* 
   return CF_OK;
 }
 
-static int toon_launch(cf_ctx* ctx, cf_batch* b, uint32_t flags, uint8_t* d_out, uint32_t* d_out_len, int32_t* d_status, const uint8_t* d_unit_stages,
-                       cudaStream_t st) {
-  uint64_t need = (b->nbytes / 2 + 4ull * b->n + 8) * sizeof(cfj::JNode);
-  const uint64_t need_tp = (b->nbytes / 2 + (uint64_t)TP_TOK_SLACK * b->n + 8) * sizeof(cftp::GTok);
-  if (need_tp > need) need = need_tp;
+// TOON device workspace: token / DOM scratch, and the first pass's unit order with the sort behind it (indices | keys in | keys out |
+// radix-sort temp storage).  The context's for cf_toon / cf_chain, a run's own for cf_run_enqueue.
+struct ToonWs {
+  void* scratch;
+  uint64_t scratch_bytes;
+  uint32_t* order;
+  uint8_t* sort;
+  size_t sort_bytes;
+};
+static uint64_t toon_scratch_need(uint64_t nbytes, uint32_t n) {
+  const uint64_t need = (nbytes / 2 + 4ull * n + 8) * sizeof(cfj::JNode);
+  const uint64_t need_tp = (nbytes / 2 + (uint64_t)TP_TOK_SLACK * n + 8) * sizeof(cftp::GTok);
+  return need_tp > need ? need_tp : need;
+}
+static size_t toon_sort_tmp_offset(uint32_t n) { return ((size_t)n * 4 + 2 * (size_t)n + 255) & ~(size_t)255; }
+static int toon_sort_temp(cf_ctx* ctx, uint32_t n, cudaStream_t st, size_t* bytes) {
+  CF_CUDA(ctx, cub::DeviceRadixSort::SortPairsDescending(nullptr, *bytes, (const uint8_t*)nullptr, (uint8_t*)nullptr, (const uint32_t*)nullptr,
+                                                         (uint32_t*)nullptr, (int)n, 0, 8, st));
+  return CF_OK;
+}
+static int toon_tp_prepare(cf_ctx* ctx) {
+  static bool smem_set = false;
+  if (!smem_set) {
+    CF_CUDA(ctx, cudaFuncSetAttribute(toon_tp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TP_SMEM));
+    smem_set = true;
+  }
+  return CF_OK;
+}
+
+// does `ws` hold the TOON stage of batch b (token-parallel path)?  Host-only, no launch.
+static int toon_ws_check(cf_ctx* ctx, const cf_batch* b, const ToonWs& ws, cudaStream_t st) {
+  size_t sort_tmp = 0;
+  int rc;
+  if ((rc = toon_sort_temp(ctx, b->n, st, &sort_tmp))) return rc;
+  if (toon_scratch_need(b->nbytes, b->n) > ws.scratch_bytes || toon_sort_tmp_offset(b->n) + sort_tmp > ws.sort_bytes) { ctx->err = "TOON workspace too small"; return CF_E_CAPACITY; }
+  return CF_OK;
+}
+
+// the TOON launches on `st` with a workspace that is already large enough (no allocation, no synchronisation)
+static int toon_enqueue(cf_ctx* ctx, cf_batch* b, uint32_t flags, uint8_t* d_out, uint32_t* d_out_len, int32_t* d_status, const uint8_t* d_unit_stages,
+                        cudaStream_t st, const ToonWs& ws) {
+  const bool tp = !(flags & (CF_TOON_PARSE_ONLY | CF_TOON_SEQUENTIAL));
+  if (!tp && d_unit_stages) { ctx->err = "per-unit stage masks need the token-parallel encoder"; return CF_E_BADARG; }
+  // the first pass's unit order: key + stable radix sort over its 8 bits, descending
+  const size_t o_kin = (size_t)b->n * 4, o_kout = o_kin + b->n, o_tmp = toon_sort_tmp_offset(b->n);
+  size_t sort_tmp = 0;
+  int rc;
+  if (tp && (rc = toon_sort_temp(ctx, b->n, st, &sort_tmp))) return rc;
+  if (toon_scratch_need(b->nbytes, b->n) > ws.scratch_bytes || (tp && o_tmp + sort_tmp > ws.sort_bytes)) { ctx->err = "TOON workspace too small"; return CF_E_CAPACITY; }
+  const bool prof = ctx->prof_on && (size_t)ctx->prof_used + 2 <= ctx->prof_ev.size();
+  if (prof) cudaEventRecord(ctx->prof_ev[ctx->prof_used], st);
+  if (tp) {
+    if ((rc = toon_tp_prepare(ctx))) return rc;
+    uint8_t* srt = ws.sort;
+    toon_order_kernel<<<(b->n + 7) / 8, 256, 0, st>>>(b->d_buf + cf::FRONT_PAD, b->d_offsets, b->n, d_unit_stages, srt + o_kin, (uint32_t*)srt);
+    ctx->launches++;
+    CF_CUDA(ctx, cudaGetLastError());
+    CF_CUDA(ctx, cub::DeviceRadixSort::SortPairsDescending(srt + o_tmp, sort_tmp, srt + o_kin, srt + o_kout, (const uint32_t*)srt, ws.order, (int)b->n, 0, 8, st));
+    ctx->launches++;
+    const uint32_t grid = (b->n + TP_WARPS - 1) / TP_WARPS;
+    toon_tp_kernel<<<grid, TP_WARPS * 32, TP_SMEM, st>>>(b->d_buf + cf::FRONT_PAD, b->d_offsets, b->n, (cftp::GTok*)ws.scratch, d_out, d_out_len,
+                                                         d_status, flags, d_unit_stages, ws.order);
+    ctx->launches++;
+    CF_CUDA(ctx, cudaGetLastError());
+    // the units the fast path handed over: sequential encoder, one unit per warp (they are few)
+    if (!(flags & CF_TOON_NO_HANDOVER)) cf_launch_toon_seq(json_blocks(b->n, 1), st, b->d_buf + cf::FRONT_PAD, b->d_offsets, b->n, (cfj::JNode*)ws.scratch, d_out, d_out_len, d_status,
+                                                     (flags & 1u) | TOON_ONLY_FALLBACK, 1);
+  } else {
+    const uint32_t upw = units_per_warp(ctx, b->n);
+    cf_launch_toon_seq(json_blocks(b->n, upw), st, b->d_buf + cf::FRONT_PAD, b->d_offsets, b->n, (cfj::JNode*)ws.scratch, d_out, d_out_len,
+                                                       d_status, flags & ~TOON_ONLY_FALLBACK, upw);
+  }
+  if (prof) { cudaEventRecord(ctx->prof_ev[ctx->prof_used + 1], st); ctx->prof_used += 2; }
+  ctx->launches++;
+  CF_CUDA(ctx, cudaGetLastError());
+  return CF_OK;
+}
+
+// the context's TOON workspace (cf_toon, cf_chain, cf_run_batch), grown on demand
+static int toon_ctx_ws(cf_ctx* ctx, const cf_batch* b, uint32_t flags, cudaStream_t st, ToonWs* ws) {
+  const uint64_t need = toon_scratch_need(b->nbytes, b->n);
   if (need > ctx->toon_scratch_bytes) {
     CF_CUDA(ctx, cudaStreamSynchronize(st));
     cudaFree(ctx->d_toon_scratch);
@@ -272,50 +352,21 @@ static int toon_launch(cf_ctx* ctx, cf_batch* b, uint32_t flags, uint8_t* d_out,
     CF_CUDA(ctx, cudaMalloc(&ctx->d_toon_scratch, need + need / 4));
     ctx->toon_scratch_bytes = need + need / 4;
   }
-  const bool tp = !(flags & (CF_TOON_PARSE_ONLY | CF_TOON_SEQUENTIAL));
-  // the first pass's unit order: key + stable radix sort over its 8 bits, descending; toon_sort = indices | keys in | keys out | temp
-  const size_t o_kin = (size_t)b->n * 4, o_kout = o_kin + b->n, o_tmp = (o_kout + b->n + 255) & ~(size_t)255;
-  size_t sort_tmp = 0;
-  if (tp) {
-    CF_CUDA(ctx, cub::DeviceRadixSort::SortPairsDescending(nullptr, sort_tmp, (const uint8_t*)nullptr, (uint8_t*)nullptr, (const uint32_t*)nullptr,
-                                                           (uint32_t*)nullptr, (int)b->n, 0, 8, st));
+  if (!(flags & (CF_TOON_PARSE_ONLY | CF_TOON_SEQUENTIAL))) {
+    size_t sort_tmp = 0;
     int rc;
+    if ((rc = toon_sort_temp(ctx, b->n, st, &sort_tmp))) return rc;
     if ((rc = cf_dev_reserve(ctx, ctx->toon_order, (size_t)b->n * 4))) return rc;
-    if ((rc = cf_dev_reserve(ctx, ctx->toon_sort, o_tmp + sort_tmp))) return rc;
+    if ((rc = cf_dev_reserve(ctx, ctx->toon_sort, toon_sort_tmp_offset(b->n) + sort_tmp))) return rc;
   }
-  const bool prof = ctx->prof_on && (size_t)ctx->prof_used + 2 <= ctx->prof_ev.size();
-  if (prof) cudaEventRecord(ctx->prof_ev[ctx->prof_used], st);
-  if (tp) {
-    static bool smem_set = false;
-    if (!smem_set) {
-      CF_CUDA(ctx, cudaFuncSetAttribute(toon_tp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TP_SMEM));
-      smem_set = true;
-    }
-    uint8_t* srt = (uint8_t*)ctx->toon_sort.p;
-    uint32_t* order = (uint32_t*)ctx->toon_order.p;
-    toon_order_kernel<<<(b->n + 7) / 8, 256, 0, st>>>(b->d_buf + cf::FRONT_PAD, b->d_offsets, b->n, d_unit_stages, srt + o_kin, (uint32_t*)srt);
-    ctx->launches++;
-    CF_CUDA(ctx, cudaGetLastError());
-    CF_CUDA(ctx, cub::DeviceRadixSort::SortPairsDescending(srt + o_tmp, sort_tmp, srt + o_kin, srt + o_kout, (const uint32_t*)srt, order, (int)b->n, 0, 8, st));
-    ctx->launches++;
-    const uint32_t grid = (b->n + TP_WARPS - 1) / TP_WARPS;
-    toon_tp_kernel<<<grid, TP_WARPS * 32, TP_SMEM, st>>>(b->d_buf + cf::FRONT_PAD, b->d_offsets, b->n, (cftp::GTok*)ctx->d_toon_scratch, d_out, d_out_len,
-                                                         d_status, flags, d_unit_stages, order);
-    ctx->launches++;
-    CF_CUDA(ctx, cudaGetLastError());
-    // the units the fast path handed over: sequential encoder, one unit per warp (they are few)
-    if (!(flags & CF_TOON_NO_HANDOVER)) cf_launch_toon_seq(json_blocks(b->n, 1), st, b->d_buf + cf::FRONT_PAD, b->d_offsets, b->n, (cfj::JNode*)ctx->d_toon_scratch, d_out, d_out_len, d_status,
-                                                     (flags & 1u) | TOON_ONLY_FALLBACK, 1);
-  } else {
-    if (d_unit_stages) { ctx->err = "per-unit stage masks need the token-parallel encoder"; return CF_E_BADARG; }
-    const uint32_t upw = units_per_warp(ctx, b->n);
-    cf_launch_toon_seq(json_blocks(b->n, upw), st, b->d_buf + cf::FRONT_PAD, b->d_offsets, b->n, (cfj::JNode*)ctx->d_toon_scratch, d_out, d_out_len,
-                                                       d_status, flags & ~TOON_ONLY_FALLBACK, upw);
-  }
-  if (prof) { cudaEventRecord(ctx->prof_ev[ctx->prof_used + 1], st); ctx->prof_used += 2; }
-  ctx->launches++;
-  CF_CUDA(ctx, cudaGetLastError());
+  *ws = ToonWs{ctx->d_toon_scratch, ctx->toon_scratch_bytes, (uint32_t*)ctx->toon_order.p, (uint8_t*)ctx->toon_sort.p, ctx->toon_sort.cap};
   return CF_OK;
+}
+static int toon_launch(cf_ctx* ctx, cf_batch* b, uint32_t flags, uint8_t* d_out, uint32_t* d_out_len, int32_t* d_status, const uint8_t* d_unit_stages,
+                       cudaStream_t st) {
+  ToonWs ws;
+  const int rc = toon_ctx_ws(ctx, b, flags, st, &ws);
+  return rc ? rc : toon_enqueue(ctx, b, flags, d_out, d_out_len, d_status, d_unit_stages, st, ws);
 }
 
 int cf_toon(cf_ctx* ctx, cf_batch* b, uint32_t flags, uint8_t* d_out, uint32_t* d_out_len, int32_t* d_status, void* cuda_stream) {
@@ -458,14 +509,84 @@ int cf_classify_keys_host(cf_ctx* ctx, cf_batch* b, const uint8_t* stream, uint6
 }
 
 
-// gather of every text cf_run_batch produced: dst[out_off[u], out_off[u+1]) = src[u][0, len), one warp per unit.  16-byte stores;
-// 16-byte loads when source and destination share their alignment, otherwise aligned 4-byte loads funnel-shifted into place.  Every
-// word loaded holds at least one byte of the source span, so no load leaves the span's 4-byte-aligned envelope.
+// ------------------------------------------------------------------------------------------------
+// the fused chain on the caller's stream (cf_run_enqueue / cf_run_finish, include/cfgpu.h).  Stream st: scan, TOON, verdicts,
+// offsets, gather.  The run's side stream: dirty-unit selection + substitution, which need only the scan's bitmaps and so run
+// beside the TOON kernel.  Nothing between the first launch and the return reads device memory on the host.
+// ------------------------------------------------------------------------------------------------
+
+// verdict records of cf_run_batch's semantics, and per unit the source and length of its produced text (len[n] = 0, so that the
+// exclusive scan of len gives out_offsets[0..n]).  A dirty unit whose substitution did not run (RUN_DEFER_PENDING) or outgrew its
+// bound (SUB_OVERFLOW) is deferred: appended to `deferred`, slot[u] = RUN_DEFER | its index there, no output yet.  cf_run_finish runs
+// the kernel again with def_rec: the deferred units' records from the synchronous substitution (offsets relative to def_base).
+__global__ void __launch_bounds__(256) run_verdict_kernel(uint32_t n, uint32_t stage_mask, const uint8_t* __restrict__ unit_stages,
+                                                          const uint64_t* __restrict__ bm, uint32_t W, const uint32_t* __restrict__ toon_ls,
+                                                          uint32_t* slot, const uint64_t* __restrict__ rec, const uint8_t* arena,
+                                                          const uint64_t* __restrict__ def_rec, const uint8_t* def_base, const uint8_t* stream,
+                                                          const uint64_t* __restrict__ offsets, const uint8_t* toon_out, uint32_t* __restrict__ deferred,
+                                                          RunStatus* st, cf_verdict* __restrict__ v, uint64_t* __restrict__ src, uint64_t* __restrict__ len) {
+  const uint32_t u = blockIdx.x * blockDim.x + threadIdx.x;
+  if (u == n) len[n] = 0;
+  if (u >= n) return;
+  uint32_t flags = 0, out_len = 0;
+  int32_t aux = 0;
+  uintptr_t s = 0;
+  const bool toon = (stage_mask & CF_STAGE_TOON) && (!unit_stages || (unit_stages[u] & CF_STAGE_TOON));
+  const uint32_t sl = slot ? slot[u] : RUN_NOT_DIRTY;
+  if (sl != RUN_NOT_DIRTY) {
+    flags = CF_V_REWRITTEN | (toon ? CF_V_RESUBMIT : 0u);    // the caller TOON-encodes the rewritten text
+    uint64_t at = SUB_OVERFLOW, l = 0;
+    const uint8_t* base = arena;
+    bool defer = sl == RUN_DEFER_PENDING;
+    if (!defer && (sl & RUN_DEFER)) {
+      if (def_rec) { at = def_rec[2 * (uint64_t)(sl & ~RUN_DEFER)]; l = def_rec[2 * (uint64_t)(sl & ~RUN_DEFER) + 1]; base = def_base; }
+    } else if (!defer) {
+      at = rec[2 * (uint64_t)sl];
+      l = rec[2 * (uint64_t)sl + 1];
+      defer = at == SUB_OVERFLOW;
+    }
+    if (defer) {
+      const uint32_t k = atomicAdd(&st->n_deferred, 1u);
+      deferred[k] = u;
+      slot[u] = RUN_DEFER | k;
+    } else if (at != SUB_OVERFLOW) {
+      s = at == ~0ull ? (uintptr_t)(stream + offsets[u]) : (uintptr_t)(base + at);
+      out_len = (uint32_t)l;
+    }
+  }
+  if (stage_mask & CF_STAGE_TOON) {
+    aux = (flags & CF_V_RESUBMIT) ? CF_TOON_SKIPPED : (int32_t)toon_ls[n + u];
+    if (aux == CF_TOON_CONVERTED && !(flags & CF_V_REWRITTEN)) {
+      flags |= CF_V_TOON;
+      out_len = toon_ls[u];
+      s = (uintptr_t)(toon_out + offsets[u]);
+    }
+  }
+  cf_verdict r;
+  r.match_bitmap = bm ? bm[(uint64_t)u * W] : 0;
+  r.flags = flags;
+  r.out_len = out_len;
+  r.aux = aux;
+  r.reserved = 0;
+  v[u] = r;
+  src[u] = s;
+  len[u] = out_len;
+}
+
+// gather of every produced text: dst[out_off[u], out_off[u+1]) = src[u][0, len), one warp per unit.  16-byte stores; 16-byte loads
+// when source and destination share their alignment, otherwise aligned 4-byte loads funnel-shifted into place.  Every word loaded
+// holds at least one byte of the source span, so no load leaves the span's 4-byte-aligned envelope.  When the total exceeds out_cap
+// nothing is written and the status block says so.
 __global__ void __launch_bounds__(256) gather_kernel(const uint64_t* __restrict__ out_off, const uint64_t* __restrict__ src, uint8_t* __restrict__ out,
-                                                     uint32_t n_units) {
+                                                     uint32_t n_units, uint64_t out_cap, RunStatus* st) {
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t u = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  if (u >= n_units) return;
+  const uint64_t total = out_off[n_units];
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    st->needed = total;
+    if (total > out_cap) st->err = CF_E_CAPACITY;
+  }
+  if (total > out_cap || u >= n_units) return;
   uint64_t n = out_off[u + 1] - out_off[u];
   if (!n) return;
   const uint8_t* s = reinterpret_cast<const uint8_t*>(src[u]);
@@ -491,10 +612,284 @@ __global__ void __launch_bounds__(256) gather_kernel(const uint64_t* __restrict_
   if (lane < n - t) d[t + lane] = s[t + lane];
 }
 
-// ---- the fused chain with host buffers (include/cfgpu.h): one H2D of the stream, every stage on the resident batch, then
-// verdicts + only the produced texts cross PCIe back.  Legacy stream: scan, TOON, gather.  ctx->side: the substitution of the units a
-// rule matched, which needs only the scan's bitmaps and so runs beside the TOON kernel.  Host <-> device copies go through the
-// context's pinned staging.
+// the gather of the run's last enqueue into run->d_out (run->out_cap bytes)
+static int run_gather(cf_ctx* ctx, cf_run* run) {
+  const uint32_t n = run->batch->n;
+  CF_CUDA(ctx, cudaMemsetAsync(&run->d_status->err, 0, sizeof(int32_t), run->st));
+  gather_kernel<<<(n + 7) / 8, 256, 0, run->st>>>(run->d_out_offsets, run->d_src, run->d_out, n, run->out_cap, run->d_status);
+  ctx->launches++;
+  CF_CUDA(ctx, cudaGetLastError());
+  return CF_OK;
+}
+
+// verdict records, out_offsets (exclusive scan of the lengths) and the gather of the run's last enqueue
+static int run_assemble(cf_ctx* ctx, cf_run* run, const uint64_t* def_rec, const uint8_t* def_base) {
+  cf_batch* b = run->batch;
+  const uint32_t n = b->n;
+  run_verdict_kernel<<<(n + 256) / 256, 256, 0, run->st>>>(n, run->stage_mask, run->d_unit_stages, run->d_bitmaps, run->W, run->d_toon_ls,
+                                                           run->sub ? run->d_slot : nullptr, run->d_rec, run->enq_arena, def_rec, def_base,
+                                                           b->d_buf + cf::FRONT_PAD, b->d_offsets, run->d_toon_out, run->d_deferred, run->d_status,
+                                                           run->d_verdicts, run->d_src, run->d_len);
+  ctx->launches++;
+  CF_CUDA(ctx, cudaGetLastError());
+  size_t tmp = 0;
+  CF_CUDA(ctx, cub::DeviceScan::ExclusiveSum(nullptr, tmp, (const uint64_t*)run->d_len, run->d_out_offsets, (int)n + 1, run->st));
+  if (tmp > run->scan_tmp_bytes) { ctx->err = "offset scan workspace too small"; return CF_E_CAPACITY; }
+  CF_CUDA(ctx, cub::DeviceScan::ExclusiveSum(run->d_scan_tmp, tmp, (const uint64_t*)run->d_len, run->d_out_offsets, (int)n + 1, run->st));
+  ctx->launches++;
+  return run_gather(ctx, run);
+}
+
+// device -> host copy on the run's side stream (non-blocking and idle once ev_done has completed), so that a finish never waits for
+// work the caller has queued on other streams since
+static int run_d2h(cf_ctx* ctx, cf_run* run, void* dst, const void* src, size_t bytes) {
+  CF_CUDA(ctx, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, run->side));
+  CF_CUDA(ctx, cudaStreamSynchronize(run->side));
+  return CF_OK;
+}
+
+// cf_run_finish without the arena's growth: cf_run_batch may gather again (into a larger buffer) from the arena first.  h_offsets:
+// the host copy of the batch's offsets that sizes the deferred units' scratch (NULL: read them from the device).  *out_short is set
+// when, and only when, CF_E_CAPACITY means the gather's output buffer: every error of the deferred units' substitution (its own
+// CF_E_CAPACITY limits included) is returned as that substitution returned it.
+static int run_finish(cf_ctx* ctx, cf_run* run, const uint64_t* h_offsets, uint64_t* needed, bool* out_short) {
+  *out_short = false;
+  if (!ctx || !run || run->ctx != ctx) return CF_E_BADARG;
+  if (!run->batch) { ctx->err = "cf_run_finish: nothing was enqueued on this run"; return CF_E_BADARG; }
+  CF_CUDA(ctx, cudaEventSynchronize(run->ev_done));
+  int rc;
+  if ((rc = run_d2h(ctx, run, run->h_status, run->d_status, sizeof(RunStatus)))) return rc;
+  if (const uint32_t nd = run->h_status->n_deferred) {
+    // the deferred units through the synchronous substitution (regrowth, CF_E_TOO_LARGE), then verdicts, offsets and gather again
+    cf_batch* b = run->batch;
+    std::vector<uint32_t> units(nd);
+    if ((rc = run_d2h(ctx, run, units.data(), run->d_deferred, (size_t)nd * 4))) return rc;
+    std::vector<uint64_t> offs;
+    if (!h_offsets) {
+      offs.resize((size_t)b->n + 1);
+      if ((rc = run_d2h(ctx, run, offs.data(), b->d_offsets, ((size_t)b->n + 1) * 8))) return rc;
+      h_offsets = offs.data();
+    }
+    if ((rc = cf_stage_reserve(ctx, cf_sub_stage_bytes(nd)))) return rc;
+    const uint64_t* rec = nullptr;
+    if ((rc = cf_sub_device(ctx, run->prog, b, h_offsets, units.data(), nd, run->st, (uint8_t*)ctx->h_stage, &rec))) return rc;
+    CF_CUDA(ctx, cudaMemcpyAsync(run->d_def_rec, rec, (size_t)nd * 16, cudaMemcpyHostToDevice, run->st));
+    if ((rc = run_assemble(ctx, run, run->d_def_rec, (const uint8_t*)ctx->tmp[8].p))) return rc;
+    CF_CUDA(ctx, cudaStreamSynchronize(run->st));
+    if ((rc = run_d2h(ctx, run, run->h_status, run->d_status, sizeof(RunStatus)))) return rc;
+  }
+  if (needed) *needed = run->h_status->needed;
+  if (run->h_status->err) { ctx->err = "output buffer too small"; *out_short = true; return CF_E_CAPACITY; }
+  return CF_OK;
+}
+
+// the arena for the next call: what this one asked for, and a quarter more.  Once an enqueue of this run was captured in a CUDA graph,
+// the graph holds the arena's address: the old arena then stays allocated until cf_run_free, so that a replay never writes freed memory.
+static int run_grow_arena(cf_ctx* ctx, cf_run* run) {
+  const uint64_t used = run->h_status->arena_used;
+  if (used <= run->arena_bytes) return CF_OK;
+  if (run->ever_captured) run->retired.push_back(run->d_arena);
+  else cudaFree(run->d_arena);
+  run->d_arena = nullptr;
+  run->arena_bytes = 0;
+  CF_CUDA(ctx, cudaMalloc(&run->d_arena, used + used / 4));
+  run->arena_bytes = used + used / 4;
+  return CF_OK;
+}
+
+// own_toon == false: the run gets no TOON workspace of its own; cf_run_batch lends it the context's before each enqueue
+static int run_create(cf_ctx* ctx, uint32_t max_units, uint64_t max_stream_bytes, uint64_t sub_arena_bytes, bool own_toon, cf_run** out) {
+  if (!ctx || !out || !max_units) return CF_E_BADARG;
+  *out = nullptr;
+  CF_CUDA(ctx, cudaSetDevice(ctx->device));
+  cf_run* r = new (std::nothrow) cf_run();
+  if (!r) return CF_E_NOMEM;
+  r->ctx = ctx;
+  r->max_units = max_units;
+  r->max_bytes = max_stream_bytes;
+  struct Guard { cf_run*& r; ~Guard() { if (r) cf_run_free(r); } } guard{r};   // every error return frees what was made
+  const uint32_t n = max_units;
+  int rc;
+  auto dev = [&](auto** p, size_t bytes) -> int {
+    void* q = nullptr;
+    CF_CUDA(ctx, cudaMalloc(&q, bytes ? bytes : 16));
+    r->allocs.push_back(q);
+    *p = reinterpret_cast<std::remove_pointer_t<decltype(p)>>(q);
+    return CF_OK;
+  };
+  if (own_toon) {
+    r->toon_scratch_bytes = toon_scratch_need(max_stream_bytes, n);
+    size_t sort_tmp = 0;
+    if ((rc = toon_sort_temp(ctx, n, nullptr, &sort_tmp))) return rc;
+    r->toon_sort_bytes = toon_sort_tmp_offset(n) + sort_tmp;
+    if ((rc = dev(&r->d_toon_scratch, r->toon_scratch_bytes)) || (rc = dev(&r->d_toon_order, (size_t)n * 4)) || (rc = dev(&r->d_toon_sort, r->toon_sort_bytes)) ||
+        (rc = dev(&r->d_toon_out, max_stream_bytes + 16)) || (rc = dev(&r->d_toon_ls, (size_t)n * 8)))
+      return rc;
+  }
+  CF_CUDA(ctx, cub::DeviceScan::ExclusiveSum(nullptr, r->scan_tmp_bytes, (const uint64_t*)nullptr, (uint64_t*)nullptr, (int)n + 1));
+  if ((rc = dev(&r->d_queue, (size_t)ctx->qcap * 8)) || (rc = dev(&r->d_qstate, 32)) || (rc = dev(&r->d_slot, (size_t)n * 4)) || (rc = dev(&r->d_sel, (size_t)n * 4)) ||
+      (rc = dev(&r->d_soff, (size_t)n * 8)) || (rc = dev(&r->d_bound, (size_t)n * 8)) || (rc = dev(&r->d_rec, (size_t)n * 16)) ||
+      (rc = dev(&r->d_deferred, (size_t)n * 4)) || (rc = dev(&r->d_def_rec, (size_t)n * 16)) || (rc = dev(&r->d_src, (size_t)n * 8)) ||
+      (rc = dev(&r->d_len, ((size_t)n + 1) * 8)) || (rc = dev(&r->d_scan_tmp, r->scan_tmp_bytes)) || (rc = dev(&r->d_status, sizeof(RunStatus))))
+    return rc;
+  CF_CUDA(ctx, cudaMemset(r->d_qstate, 0, 32));
+  CF_CUDA(ctx, cudaMemset(r->d_status, 0, sizeof(RunStatus)));
+  if (sub_arena_bytes) {
+    CF_CUDA(ctx, cudaMalloc(&r->d_arena, sub_arena_bytes));
+    r->arena_bytes = sub_arena_bytes;
+  }
+  CF_CUDA(ctx, cudaHostAlloc((void**)&r->h_status, sizeof(RunStatus), cudaHostAllocDefault));
+  memset(r->h_status, 0, sizeof(RunStatus));
+  int prio_lo = 0, prio_hi = 0;   // the few substitution blocks take SMs as TOON blocks retire instead of queueing behind all of them
+  CF_CUDA(ctx, cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
+  CF_CUDA(ctx, cudaStreamCreateWithPriority(&r->side, cudaStreamNonBlocking, prio_hi));
+  for (cudaEvent_t* e : {&r->ev_scan, &r->ev_sub, &r->ev_done}) CF_CUDA(ctx, cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+  if ((rc = toon_tp_prepare(ctx))) return rc;
+  *out = r;
+  r = nullptr;
+  return CF_OK;
+}
+int cf_run_create(cf_ctx* ctx, uint32_t max_units, uint64_t max_stream_bytes, uint64_t sub_arena_bytes, cf_run** out) {
+  return run_create(ctx, max_units, max_stream_bytes, sub_arena_bytes, true, out);
+}
+
+void cf_run_free(cf_run* run) {
+  if (!run) return;
+  cudaSetDevice(run->ctx->device);
+  if (run->side) cudaStreamSynchronize(run->side);
+  for (void* p : run->allocs) cudaFree(p);
+  cudaFree(run->d_arena);
+  for (void* p : run->retired) cudaFree(p);
+  if (run->h_status) cudaFreeHost(run->h_status);
+  if (run->side) cudaStreamDestroy(run->side);
+  for (cudaEvent_t e : {run->ev_scan, run->ev_sub, run->ev_done}) if (e) cudaEventDestroy(e);
+  delete run;
+}
+
+int cf_run_enqueue(cf_ctx* ctx, cf_prog* prog, cf_batch* b, cf_run* run, uint32_t stage_mask, const uint8_t* d_unit_stages, uint32_t toon_flags,
+                   cf_verdict* d_verdicts, uint64_t* d_bitmaps_full, uint64_t* d_out_offsets, uint8_t* d_out, uint64_t out_cap, void* cuda_stream) {
+  if (!ctx || !b || !run || run->ctx != ctx || !d_verdicts || !d_out_offsets || (!d_out && out_cap)) return CF_E_BADARG;
+  if (stage_mask & CF_STAGE_MASK) { ctx->err = "cf_run_enqueue runs CF_STAGE_SCAN / SUB / TOON; masking needs cf_run_batch"; return CF_E_BADARG; }
+  if (stage_mask & ~(CF_STAGE_SCAN | CF_STAGE_SUB | CF_STAGE_TOON)) { ctx->err = "unknown stage bits"; return CF_E_BADARG; }
+  if (stage_mask & CF_STAGE_SUB) stage_mask |= CF_STAGE_SCAN;
+  if ((stage_mask & CF_STAGE_SCAN) && (!prog || !d_bitmaps_full)) { ctx->err = "CF_STAGE_SCAN / SUB need a program and d_bitmaps_full"; return CF_E_BADARG; }
+  const uint32_t n = b->n;
+  if (!n) { ctx->err = "the batch holds no units"; return CF_E_BADARG; }
+  if (n > run->max_units || b->nbytes > run->max_bytes) { ctx->err = "the batch exceeds the run's max_units / max_stream_bytes"; return CF_E_CAPACITY; }
+  cudaStream_t st = (cudaStream_t)cuda_stream;
+  // every check that can fail comes before the first launch, so that an error return leaves nothing queued
+  int rc;
+  const ToonWs ws{run->d_toon_scratch, run->toon_scratch_bytes, run->d_toon_order, run->d_toon_sort, run->toon_sort_bytes};
+  if (stage_mask & CF_STAGE_TOON) {
+    if (!run->d_toon_scratch || !run->d_toon_out) { ctx->err = "the run has no TOON workspace"; return CF_E_BADARG; }
+    if ((rc = toon_ws_check(ctx, b, ws, st))) return rc;
+  }
+  size_t scan_tmp = 0;
+  CF_CUDA(ctx, cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (const uint64_t*)nullptr, (uint64_t*)nullptr, (int)n + 1, st));
+  if (scan_tmp > run->scan_tmp_bytes) { ctx->err = "offset scan workspace too small"; return CF_E_CAPACITY; }
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  CF_CUDA(ctx, cudaStreamIsCapturing(st, &cs));
+  if (cs == cudaStreamCaptureStatusActive) run->ever_captured = true;
+  run->prog = prog;
+  run->batch = b;
+  run->st = st;
+  run->stage_mask = stage_mask;
+  run->d_unit_stages = d_unit_stages;
+  run->d_verdicts = d_verdicts;
+  run->d_bitmaps = (stage_mask & CF_STAGE_SCAN) ? d_bitmaps_full : nullptr;
+  run->d_out_offsets = d_out_offsets;
+  run->d_out = d_out;
+  run->out_cap = out_cap;
+  run->W = prog ? prog->W : 1;
+  run->sub = (stage_mask & CF_STAGE_SUB) && !prog->ordered.empty();
+  run->enq_arena = run->d_arena;      // a finish after a replay of this enqueue must read the arena the graph holds, even once grown
+  CF_CUDA(ctx, cudaMemsetAsync(run->d_status, 0, sizeof(RunStatus), st));
+  if ((stage_mask & CF_STAGE_SCAN) && (rc = cf_scan_launch(ctx, prog, b, d_bitmaps_full, st, run->d_queue, run->d_qstate, &run->qphase))) return rc;
+  if (run->sub) {
+    CF_CUDA(ctx, cudaEventRecord(run->ev_scan, st));
+    CF_CUDA(ctx, cudaStreamWaitEvent(run->side, run->ev_scan, 0));
+    if ((rc = cf_sub_enqueue(ctx, prog, b, run, d_bitmaps_full, d_unit_stages, run->side))) return rc;
+    CF_CUDA(ctx, cudaEventRecord(run->ev_sub, run->side));
+  }
+  if (stage_mask & CF_STAGE_TOON) {
+    if ((rc = toon_enqueue(ctx, b, toon_flags & ~(CF_TOON_PARSE_ONLY | CF_TOON_SEQUENTIAL | CF_RUN_OUTPUTS_RESIDENT), run->d_toon_out, run->d_toon_ls,
+                           (int32_t*)(run->d_toon_ls + n), d_unit_stages, st, ws))) return rc;
+  }
+  if (run->sub) CF_CUDA(ctx, cudaStreamWaitEvent(st, run->ev_sub, 0));
+  if ((rc = run_assemble(ctx, run, nullptr, nullptr))) return rc;
+  // inside a stream capture the completion event becomes a node of the graph, so that cf_run_finish waits for each replay
+  CF_CUDA(ctx, cudaEventRecordWithFlags(run->ev_done, st, cs == cudaStreamCaptureStatusActive ? cudaEventRecordExternal : cudaEventRecordDefault));
+  return CF_OK;
+}
+
+int cf_run_finish(cf_ctx* ctx, cf_run* run, uint64_t* needed) {
+  if (needed) *needed = 0;
+  bool out_short = false;
+  int rc = run_finish(ctx, run, nullptr, needed, &out_short);
+  if (rc == CF_E_CAPACITY && !out_short) rc = CF_E_TOO_LARGE;   // a deferred unit's substitution hit one of its limits: not the output buffer
+  if (ctx && run && run->ctx == ctx) {
+    const int g = run_grow_arena(ctx, run);
+    if (g && !rc) return g;
+  }
+  return rc;
+}
+
+// CF_STAGE_MASK: the scan (and the substitution's verdict flags) and request_logging_masking on one upload; the masking kernel
+// gathers its own texts.
+static int run_batch_mask(cf_ctx* ctx, cf_prog* prog, cf_batch* b, const uint8_t* stream, uint64_t stream_bytes, const uint64_t* offsets, uint32_t n_units,
+                          uint32_t stage_mask, const uint8_t* unit_stages, int mask_max_depth, cf_verdict* verdicts, uint64_t* bitmaps_full,
+                          uint8_t* out_bytes, uint64_t out_cap, uint64_t* out_offsets, uint64_t* out_needed) {
+  const uint32_t W = prog ? prog->W : 1;
+  // pinned staging: bitmaps | substitution descriptors
+  const size_t o_sub = (((stage_mask & CF_STAGE_SCAN) ? (size_t)n_units * W * 8 : 0) + 15) & ~(size_t)15;
+  int rc = cf_stage_reserve(ctx, o_sub + ((stage_mask & CF_STAGE_SUB) ? cf_sub_stage_bytes(n_units) : 0));
+  if (rc) return rc;
+  uint8_t* hs = (uint8_t*)ctx->h_stage;
+  if (stream && (rc = cf_batch_upload(ctx, b, stream, stream_bytes, offsets, n_units, nullptr))) return rc;
+  for (uint32_t i = 0; i < n_units; ++i) { verdicts[i].match_bitmap = 0; verdicts[i].flags = 0; verdicts[i].out_len = 0; verdicts[i].aux = 0; verdicts[i].reserved = 0; }
+  if (stage_mask & CF_STAGE_SCAN) {
+    const uint64_t* bm = (const uint64_t*)hs;
+    if ((rc = cf_dev_reserve(ctx, ctx->tmp[6], (size_t)n_units * W * 8))) return rc;
+    if ((rc = cf_scan(ctx, prog, b, (uint64_t*)ctx->tmp[6].p, nullptr))) return rc;
+    CF_CUDA(ctx, cudaMemcpy(hs, ctx->tmp[6].p, (size_t)n_units * W * 8, cudaMemcpyDeviceToHost));
+    if (bitmaps_full) memcpy(bitmaps_full, bm, (size_t)n_units * W * 8);
+    std::vector<uint64_t> rule_mask(W, 0);
+    for (int pi : prog->ordered_pat) rule_mask[(size_t)pi / 64] |= 1ull << (pi % 64);
+    std::vector<uint32_t> dirty;
+    for (uint32_t i = 0; i < n_units; ++i) {
+      verdicts[i].match_bitmap = bm[(size_t)i * W];
+      if ((stage_mask & CF_STAGE_SUB) && (!unit_stages || (unit_stages[i] & CF_STAGE_SUB))) {
+        bool d = false;
+        for (uint32_t w = 0; w < W; ++w) if (bm[(size_t)i * W + w] & rule_mask[w]) { d = true; break; }
+        if (d) dirty.push_back(i);
+      }
+    }
+    const uint64_t* rec = nullptr;
+    if (!dirty.empty()) {
+      if ((rc = cf_sub_device(ctx, prog, b, offsets, dirty.data(), (uint32_t)dirty.size(), 0, hs + o_sub, &rec))) return rc;
+      for (size_t k = 0; k < dirty.size(); ++k) {
+        verdicts[dirty[k]].flags |= CF_V_REWRITTEN;
+        verdicts[dirty[k]].out_len = (uint32_t)rec[2 * k + 1];
+      }
+    }
+  }
+  std::vector<int32_t> mst(n_units);
+  std::vector<uint64_t> moff((size_t)n_units + 1);
+  uint64_t need = 0;
+  rc = cf_mask_resident(ctx, b, mask_max_depth, out_bytes, out_cap, moff.data(), mst.data(), &need);
+  if (out_needed) *out_needed = need;
+  if (rc) return rc;
+  for (uint32_t i = 0; i < n_units; ++i) {
+    out_offsets[i] = moff[i];
+    verdicts[i].aux = mst[i];
+    if (mst[i] == CF_MASK_OK) { verdicts[i].flags |= CF_V_MASKED; verdicts[i].out_len = (uint32_t)(moff[i + 1] - moff[i]); }
+  }
+  out_offsets[n_units] = moff[n_units];
+  return CF_OK;
+}
+
+// ---- the fused chain with host buffers (include/cfgpu.h): one H2D of the stream, cf_run_enqueue + cf_run_finish on the context's
+// run (legacy stream), then verdicts, offsets and only the produced texts cross PCIe back through the context's pinned staging.
 int cf_run_batch(cf_ctx* ctx, cf_prog* prog, cf_batch* b, const uint8_t* stream, uint64_t stream_bytes, const uint64_t* offsets, uint32_t n_units,
                  uint32_t stage_mask, const uint8_t* unit_stages, uint32_t toon_flags, int mask_max_depth, cf_verdict* verdicts, uint64_t* bitmaps_full,
                  uint8_t* out_bytes, uint64_t out_cap, uint64_t* out_offsets, uint64_t* out_needed) {
@@ -504,24 +899,46 @@ int cf_run_batch(cf_ctx* ctx, cf_prog* prog, cf_batch* b, const uint8_t* stream,
   if (stage_mask & CF_STAGE_SUB) stage_mask |= CF_STAGE_SCAN;
   if (!stream && (b->n != n_units || b->nbytes != stream_bytes)) { ctx->err = "resident run: the batch on the device is a different one"; return CF_E_BADARG; }
   struct Nvtx { Nvtx(const char* n) { nvtxRangePushA(n); } ~Nvtx() { nvtxRangePop(); } } nvtx_call("cf_run_batch");   // ranges: assemble (caller) | h2d | kernels | d2h
-  // every return, error returns included, waits for both streams: nothing the next call's buffers are reused for stays in flight
-  struct Drain { cf_ctx* c; ~Drain() { cudaStreamSynchronize(c->side); cudaStreamSynchronize(0); } } drain{ctx};
+  // every return, error returns included, waits for the run's streams: nothing the next call's buffers are reused for stays in flight
+  struct Drain { cf_ctx* c; ~Drain() { if (c->run) cudaStreamSynchronize(c->run->side); cudaStreamSynchronize(0); } } drain{ctx};
+  if (stage_mask & CF_STAGE_MASK)
+    return run_batch_mask(ctx, prog, b, stream, stream_bytes, offsets, n_units, stage_mask, unit_stages, mask_max_depth, verdicts, bitmaps_full, out_bytes,
+                          out_cap, out_offsets, out_needed);
   const uint32_t W = prog ? prog->W : 1;
-  // pinned staging: unit_stages | bitmaps | TOON lengths + statuses | gather descriptors | substitution descriptors
-  auto r16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
-  const size_t o_bm = r16(unit_stages ? n_units : 0);
-  const size_t o_toon = o_bm + r16((stage_mask & CF_STAGE_SCAN) ? (size_t)n_units * W * 8 : 0);
-  const size_t o_gather = o_toon + r16((size_t)n_units * 8);
-  const size_t o_sub = o_gather + r16(((size_t)2 * n_units + 1) * 8);
-  int rc = cf_stage_reserve(ctx, o_sub + ((stage_mask & CF_STAGE_SUB) ? cf_sub_stage_bytes(n_units) : 0));
-  if (rc) return rc;
-  uint8_t* hs = (uint8_t*)ctx->h_stage;
+  int rc;
   if (stream) {
     nvtxRangePushA("cf_run_batch:h2d");
     rc = cf_batch_upload(ctx, b, stream, stream_bytes, offsets, n_units, nullptr);
     nvtxRangePop();
     if (rc) return rc;
   }
+  if (!ctx->run || ctx->run->max_units < n_units || ctx->run->max_bytes < stream_bytes) {     // the context's run, grown with the batches
+    const uint64_t arena = ctx->run ? ctx->run->arena_bytes : (1ull << 20);
+    cf_run_free(ctx->run);
+    ctx->run = nullptr;
+    if ((rc = run_create(ctx, n_units + n_units / 4, stream_bytes + stream_bytes / 4 + 4096, arena, false, &ctx->run))) return rc;
+  }
+  cf_run* run = ctx->run;
+  if (stage_mask & CF_STAGE_TOON) {       // the context's TOON workspace, lent to its run: TOON output in tmp[0], lengths | statuses in tmp[2]
+    ToonWs ws;
+    if ((rc = toon_ctx_ws(ctx, b, 0, 0, &ws)) || (rc = cf_dev_reserve(ctx, ctx->tmp[0], stream_bytes + 16)) ||
+        (rc = cf_dev_reserve(ctx, ctx->tmp[2], (size_t)n_units * 8)))
+      return rc;
+    run->d_toon_scratch = ws.scratch; run->toon_scratch_bytes = ws.scratch_bytes;
+    run->d_toon_order = ws.order; run->d_toon_sort = ws.sort; run->toon_sort_bytes = ws.sort_bytes;
+    run->d_toon_out = (uint8_t*)ctx->tmp[0].p;
+    run->d_toon_ls = (uint32_t*)ctx->tmp[2].p;
+  }
+  // pinned staging: unit_stages on the way in; verdicts | out_offsets | bitmaps on the way out
+  const bool keep = (toon_flags & CF_RUN_OUTPUTS_RESIDENT) != 0;
+  const size_t o_oo = ((size_t)n_units * sizeof(cf_verdict) + 15) & ~(size_t)15, o_bm = (o_oo + ((size_t)n_units + 1) * 8 + 15) & ~(size_t)15;
+  const size_t bm_bytes = (stage_mask & CF_STAGE_SCAN) ? (size_t)n_units * W * 8 : 0;
+  if ((rc = cf_stage_reserve(ctx, std::max(o_bm + bm_bytes, (size_t)n_units)))) return rc;
+  uint8_t* hs = (uint8_t*)ctx->h_stage;
+  if ((rc = cf_dev_reserve(ctx, ctx->tmp[1], (size_t)n_units * sizeof(cf_verdict))) || (rc = cf_dev_reserve(ctx, ctx->tmp[3], ((size_t)n_units + 1) * 8)) ||
+      (bm_bytes && (rc = cf_dev_reserve(ctx, ctx->tmp[6], bm_bytes))) ||
+      (rc = cf_dev_reserve(ctx, ctx->tmp[4], std::max<uint64_t>(16, keep ? stream_bytes : std::min(out_cap, stream_bytes)))))
+    return rc;
   uint8_t* d_us = nullptr;
   if (unit_stages) {
     if ((rc = cf_dev_reserve(ctx, ctx->tmp[7], n_units))) return rc;
@@ -529,108 +946,43 @@ int cf_run_batch(cf_ctx* ctx, cf_prog* prog, cf_batch* b, const uint8_t* stream,
     memcpy(hs, unit_stages, n_units);
     CF_CUDA(ctx, cudaMemcpyAsync(d_us, hs, n_units, cudaMemcpyHostToDevice, 0));
   }
-  // ---- launches, back to back; each stage's per-unit results come back in one D2H behind it
+  cf_verdict* d_v = (cf_verdict*)ctx->tmp[1].p;
+  uint64_t* d_oo = (uint64_t*)ctx->tmp[3].p;
+  // the device buffer takes what the caller can take (all of it when the texts stay resident); a shortfall of the device buffer alone
+  // is made up below by growing it and gathering again
+  const uint64_t dcap = keep ? ctx->tmp[4].cap : (out_bytes ? std::min<uint64_t>(ctx->tmp[4].cap, out_cap) : 0);
   nvtxRangePushA("cf_run_batch:kernels");
-  const uint64_t* bm = (const uint64_t*)(hs + o_bm);
-  uint32_t* tlen = (uint32_t*)(hs + o_toon);
-  const int32_t* tst = (const int32_t*)(tlen + n_units);
-  if (stage_mask & CF_STAGE_SCAN) {
-    if ((rc = cf_dev_reserve(ctx, ctx->tmp[6], (size_t)n_units * W * 8))) return rc;
-    if ((rc = cf_scan(ctx, prog, b, (uint64_t*)ctx->tmp[6].p, nullptr))) return rc;
-    CF_CUDA(ctx, cudaMemcpyAsync(hs + o_bm, ctx->tmp[6].p, (size_t)n_units * W * 8, cudaMemcpyDeviceToHost, 0));
-    CF_CUDA(ctx, cudaEventRecord(ctx->ev_scan, 0));
-  }
-  if (stage_mask & CF_STAGE_TOON) {
-    if ((rc = cf_dev_reserve(ctx, ctx->tmp[0], stream_bytes + 16))) return rc;
-    if ((rc = cf_dev_reserve(ctx, ctx->tmp[1], (size_t)n_units * 8))) return rc;     // lengths | statuses
-    uint32_t* d_len = (uint32_t*)ctx->tmp[1].p;
-    if ((rc = toon_launch(ctx, b, toon_flags & ~(CF_TOON_PARSE_ONLY | CF_TOON_SEQUENTIAL | CF_RUN_OUTPUTS_RESIDENT), (uint8_t*)ctx->tmp[0].p, d_len,
-                          (int32_t*)(d_len + n_units), d_us, 0))) return rc;
-    CF_CUDA(ctx, cudaMemcpyAsync(tlen, d_len, (size_t)n_units * 8, cudaMemcpyDeviceToHost, 0));
-    CF_CUDA(ctx, cudaEventRecord(ctx->ev_toon, 0));
-  }
-  nvtxRangePop();
-  // ---- results of the launches
-  Nvtx nvtx_d2h("cf_run_batch:d2h+verdicts");
-  for (uint32_t i = 0; i < n_units; ++i) { verdicts[i].match_bitmap = 0; verdicts[i].flags = 0; verdicts[i].out_len = 0; verdicts[i].aux = 0; verdicts[i].reserved = 0; }
-  std::vector<uint32_t> dirty;
-  if (stage_mask & CF_STAGE_SCAN) {
-    CF_CUDA(ctx, cudaEventSynchronize(ctx->ev_scan));
-    if (bitmaps_full) memcpy(bitmaps_full, bm, (size_t)n_units * W * 8);
-    std::vector<uint64_t> rule_mask(W, 0);
-    for (int pi : prog->ordered_pat) rule_mask[(size_t)pi / 64] |= 1ull << (pi % 64);
-    for (uint32_t i = 0; i < n_units; ++i) {
-      verdicts[i].match_bitmap = bm[(size_t)i * W];
-      if ((stage_mask & CF_STAGE_SUB) && (!unit_stages || (unit_stages[i] & CF_STAGE_SUB))) {
-        bool d = false;
-        for (uint32_t w = 0; w < W; ++w) if (bm[(size_t)i * W + w] & rule_mask[w]) { d = true; break; }
-        if (d) dirty.push_back(i);
-      }
-    }
-  }
-  // ---- regex_filter rewriting of the (few) units a rule matched, on the side stream while the TOON kernel runs
-  const uint64_t* rec = nullptr;
-  if (!dirty.empty()) {
-    CF_CUDA(ctx, cudaStreamWaitEvent(ctx->side, ctx->ev_scan, 0));
-    if ((rc = cf_sub_device(ctx, prog, b, offsets, dirty.data(), (uint32_t)dirty.size(), ctx->side, hs + o_sub, &rec))) return rc;
-    CF_CUDA(ctx, cudaEventRecord(ctx->ev_sub, ctx->side));
-    CF_CUDA(ctx, cudaStreamWaitEvent(0, ctx->ev_sub, 0));
-    for (size_t k = 0; k < dirty.size(); ++k) {
-      const uint32_t i = dirty[k];
-      verdicts[i].flags |= CF_V_REWRITTEN;
-      verdicts[i].out_len = (uint32_t)rec[2 * k + 1];
-      if ((stage_mask & CF_STAGE_TOON) && (!unit_stages || (unit_stages[i] & CF_STAGE_TOON))) verdicts[i].flags |= CF_V_RESUBMIT;
-    }
-  }
-  if (stage_mask & CF_STAGE_TOON) {
-    CF_CUDA(ctx, cudaEventSynchronize(ctx->ev_toon));
-    for (uint32_t i = 0; i < n_units; ++i) {
-      const int32_t s = (verdicts[i].flags & CF_V_RESUBMIT) ? CF_TOON_SKIPPED : tst[i];   // the caller encodes the rewritten text
-      verdicts[i].aux = s;
-      if (s == CF_TOON_CONVERTED && !(verdicts[i].flags & CF_V_REWRITTEN)) { verdicts[i].flags |= CF_V_TOON; verdicts[i].out_len = tlen[i]; }
-    }
-  }
-  // ---- masking on the same upload (sequential kernel; its own gather)
-  if (stage_mask & CF_STAGE_MASK) {
-    std::vector<int32_t> mst(n_units);
-    std::vector<uint64_t> moff((size_t)n_units + 1);
-    uint64_t need = 0;
-    rc = cf_mask_resident(ctx, b, mask_max_depth, out_bytes, out_cap, moff.data(), mst.data(), &need);
-    if (out_needed) *out_needed = need;
-    if (rc) return rc;
-    for (uint32_t i = 0; i < n_units; ++i) {
-      out_offsets[i] = moff[i];
-      verdicts[i].aux = mst[i];
-      if (mst[i] == CF_MASK_OK) { verdicts[i].flags |= CF_V_MASKED; verdicts[i].out_len = (uint32_t)(moff[i + 1] - moff[i]); }
-    }
-    out_offsets[n_units] = moff[n_units];
-    return CF_OK;
-  }
-  // ---- pack the outputs: TOON texts (input layout in tmp[0]) and rewritten texts (substitution scratch, or the unit itself) in one
-  // gather at their final offsets, then one D2H straight into out_bytes unless they stay resident
+  rc = cf_run_enqueue(ctx, prog, b, run, stage_mask, d_us, toon_flags, d_v, bm_bytes ? (uint64_t*)ctx->tmp[6].p : nullptr, d_oo, (uint8_t*)ctx->tmp[4].p,
+                      dcap, nullptr);
   uint64_t total = 0;
-  for (uint32_t i = 0; i < n_units; ++i) { out_offsets[i] = total; total += verdicts[i].out_len; }
-  out_offsets[n_units] = total;
-  if (out_needed) *out_needed = total;
-  const bool keep = (toon_flags & CF_RUN_OUTPUTS_RESIDENT) != 0;
-  ctx->run_out = nullptr; ctx->run_out_bytes = 0;
-  if (!keep && (total > out_cap || (!out_bytes && total))) { ctx->err = "output buffer too small"; return CF_E_CAPACITY; }
-  if (total) {
-    uint64_t* h_src = (uint64_t*)(hs + o_gather);          // src[n] | out_off[n + 1]: one H2D
-    const uintptr_t toon_out = (uintptr_t)ctx->tmp[0].p, d_stream = (uintptr_t)(b->d_buf + cf::FRONT_PAD), scratch = (uintptr_t)ctx->tmp[8].p;
-    for (uint32_t i = 0; i < n_units; ++i) h_src[i] = (verdicts[i].flags & CF_V_TOON) ? toon_out + offsets[i] : 0;
-    for (size_t k = 0; k < dirty.size(); ++k) h_src[dirty[k]] = rec[2 * k] == ~0ull ? d_stream + offsets[dirty[k]] : scratch + rec[2 * k];
-    memcpy(h_src + n_units, out_offsets, ((size_t)n_units + 1) * 8);
-    if ((rc = cf_dev_reserve(ctx, ctx->tmp[3], ((size_t)2 * n_units + 1) * 8))) return rc;
+  bool out_short = false;
+  if (!rc) rc = run_finish(ctx, run, offsets, &total, &out_short);
+  nvtxRangePop();
+  if (out_short && (keep || (out_bytes && total <= out_cap))) {
     if ((rc = cf_dev_reserve(ctx, ctx->tmp[4], total))) return rc;
-    const uint64_t* d_src = (const uint64_t*)ctx->tmp[3].p;
-    CF_CUDA(ctx, cudaMemcpyAsync(ctx->tmp[3].p, h_src, ((size_t)2 * n_units + 1) * 8, cudaMemcpyHostToDevice, 0));
-    gather_kernel<<<(n_units + 7) / 8, 256, 0, 0>>>(d_src + n_units, d_src, (uint8_t*)ctx->tmp[4].p, n_units);
-    ctx->launches++;
-    CF_CUDA(ctx, cudaGetLastError());
-    if (!keep) CF_CUDA(ctx, cudaMemcpyAsync(out_bytes, ctx->tmp[4].p, total, cudaMemcpyDeviceToHost, 0));
+    run->d_out = (uint8_t*)ctx->tmp[4].p;
+    run->out_cap = total;
+    if ((rc = run_gather(ctx, run))) return rc;
     CF_CUDA(ctx, cudaStreamSynchronize(0));
   }
+  const int grown = run_grow_arena(ctx, run);
+  if (rc && !out_short) return rc;
+  if (grown) return grown;
+  Nvtx nvtx_d2h("cf_run_batch:d2h");
+  if ((rc = cf_stage_reserve(ctx, o_bm + bm_bytes))) return rc;    // a deferred unit's substitution may have grown the staging
+  hs = (uint8_t*)ctx->h_stage;
+  CF_CUDA(ctx, cudaMemcpyAsync(hs, d_v, (size_t)n_units * sizeof(cf_verdict), cudaMemcpyDeviceToHost, 0));
+  CF_CUDA(ctx, cudaMemcpyAsync(hs + o_oo, d_oo, ((size_t)n_units + 1) * 8, cudaMemcpyDeviceToHost, 0));
+  if (bitmaps_full && bm_bytes) CF_CUDA(ctx, cudaMemcpyAsync(hs + o_bm, ctx->tmp[6].p, bm_bytes, cudaMemcpyDeviceToHost, 0));
+  const bool fits = keep || (total <= out_cap && (out_bytes || !total));
+  if (fits && !keep && total) CF_CUDA(ctx, cudaMemcpyAsync(out_bytes, ctx->tmp[4].p, total, cudaMemcpyDeviceToHost, 0));
+  CF_CUDA(ctx, cudaStreamSynchronize(0));
+  memcpy(verdicts, hs, (size_t)n_units * sizeof(cf_verdict));
+  memcpy(out_offsets, hs + o_oo, ((size_t)n_units + 1) * 8);
+  if (bitmaps_full && bm_bytes) memcpy(bitmaps_full, hs + o_bm, bm_bytes);
+  if (out_needed) *out_needed = total;
+  ctx->run_out = nullptr; ctx->run_out_bytes = 0;
+  if (!fits) { ctx->err = "output buffer too small"; return CF_E_CAPACITY; }
   if (keep) {
     ctx->run_out = total ? (const uint8_t*)ctx->tmp[4].p : nullptr;
     ctx->run_out_bytes = total;

@@ -313,6 +313,87 @@ def run_batch(prog: Optional[Program], batch: Batch, stream, offsets: np.ndarray
     return verdicts, out, out_offs, full
 
 
+def _dev_ptr(x) -> Optional[int]:
+    """Device address of a CUDA torch tensor, or a raw device pointer (int), or None."""
+    if x is None:
+        return None
+    if isinstance(x, int):
+        return x
+    if not x.is_cuda or not x.is_contiguous():
+        raise ValueError("cf_run buffers must be contiguous CUDA tensors or raw device pointers")
+    return x.data_ptr()
+
+
+class Run:
+    """cf_run: the fused chain (scan, regex_filter rewriting, TOON) enqueued on the caller's CUDA stream, with verdicts, offsets and
+    texts left in device memory.  `enqueue` returns as soon as the work is queued (it may be captured in a CUDA graph); `finish`
+    waits for it.  Each Run holds its own device state, so several can be in flight on different streams.
+
+        run = Run(ctx, max_units, max_bytes)
+        batch.upload(stream, offsets, cuda_stream=s)              # on the same stream
+        run.enqueue(prog, batch, STAGES, None, 0, verdicts, out_offsets, out, bitmaps_full, stream=s)
+        needed = run.finish()                                     # 0, or the capacity `out` needs; CfError on failure
+    """
+
+    def __init__(self, ctx: Context, max_units: int, max_bytes: int, sub_arena_bytes: int = 1 << 20):
+        self.ctx = ctx
+        self.h = c_void_p()
+        with ctx.lock:
+            ctx.check(ctx.lib.cf_run_create(ctx.h, max_units, max_bytes, sub_arena_bytes, byref(self.h)), "cf_run_create")
+        self._keep = ()
+
+    def enqueue(self, prog: Optional[Program], batch: Batch, stage_mask: int, d_unit_stages, toon_flags: int, verdicts, out_offsets, out,
+                bitmaps_full=None, stream=0) -> None:
+        """verdicts: n * 24 bytes (e.g. a uint8 / int64 tensor), out_offsets: n + 1 uint64, out: the texts' buffer (its byte size is
+        the capacity), bitmaps_full: n * W uint64 (allocated here when None and SCAN / SUB run).  Tensor sizes are checked against
+        the batch (ValueError); raw device pointers are taken as they are.  `stream`: a torch.cuda.Stream or a raw
+        cudaStream_t.  The buffers must stay alive and untouched until finish()."""
+        n = int(self.ctx.lib.cf_batch_units(batch.h))
+        scan = bool(stage_mask & (N.CF_STAGE_SCAN | N.CF_STAGE_SUB))
+        if bitmaps_full is None and scan:
+            import torch
+
+            bitmaps_full = torch.empty(n * prog.words, dtype=torch.int64, device=verdicts.device if hasattr(verdicts, "device") else "cuda")
+        if not hasattr(out, "numel"):
+            raise ValueError("pass `out` as a CUDA tensor (its byte size is the capacity)")
+        cap = out.numel() * out.element_size()
+        # the kernels write n records, n + 1 offsets and n * W bitmap words: a short tensor would be written past its end
+        for name, t, need in (("verdicts", verdicts, 24 * n), ("out_offsets", out_offsets, 8 * (n + 1)),
+                              ("bitmaps_full", bitmaps_full if scan else None, 8 * n * (prog.words if prog is not None else 1)),
+                              ("d_unit_stages", d_unit_stages, n)):
+            if t is not None and not isinstance(t, int) and t.numel() * t.element_size() < need:
+                raise ValueError(f"{name} holds {t.numel() * t.element_size()} bytes; this batch needs {need}")
+        st = getattr(stream, "cuda_stream", stream)
+        self._keep = (verdicts, out_offsets, out, bitmaps_full, d_unit_stages)
+        with self.ctx.lock:
+            self.ctx.check(self.ctx.lib.cf_run_enqueue(self.ctx.h, prog.h if prog is not None else None, batch.h, self.h, stage_mask, _dev_ptr(d_unit_stages),
+                                                       toon_flags, _dev_ptr(verdicts), _dev_ptr(bitmaps_full), _dev_ptr(out_offsets), _dev_ptr(out), cap,
+                                                       st or None), "cf_run_enqueue")
+
+    @property
+    def bitmaps_full(self):
+        """The bitmap buffer of the last enqueue (the one passed in, or the one allocated for it)."""
+        return self._keep[3] if self._keep else None
+
+    def finish(self) -> int:
+        """Wait for the last enqueue (or a graph replay of it).  Returns 0 when every text was gathered into `out`, and the bytes
+        `out` must hold when it was too small (CF_E_CAPACITY: verdicts and out_offsets are valid, `out` is untouched); raises
+        CfError on any other failure."""
+        need = c_uint64(0)
+        with self.ctx.lock:
+            rc = self.ctx.lib.cf_run_finish(self.ctx.h, self.h, byref(need))
+        if rc == N.CF_E_CAPACITY and need.value:
+            return int(need.value)
+        self.ctx.check(rc, "cf_run_finish")
+        return 0
+
+    def __del__(self):
+        try:
+            self.ctx.lib.cf_run_free(self.h)
+        except Exception:
+            pass
+
+
 def device_output(ctx: Context) -> np.ndarray:
     """Host copy of the device buffer the last `run_batch(..., outputs_resident=True)` of this context left in HBM."""
     p = c_void_p()
