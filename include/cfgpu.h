@@ -31,7 +31,6 @@
  *
  * Environment (read once per process):
  *   CF_SCAN_RESERVE_SMS=k   the persistent scan grid leaves k SMs free (a collective running beside it needs somewhere to go)
- *   CF_SCAN_WARPS / CF_SCAN_LB / CF_SCAN_ACC / CF_SCAN_STAGES   scan kernel variant (16 / 64 / 1 / 3)
  *   CF_PAIR_FILTER=0|1   force the byte / pair prefilter instead of choosing per rule set (tests, measurements)
  *
  * Conventions: every function returns CF_OK (0) or a negative CF_E_* code and never throws.

@@ -15,10 +15,17 @@
 // ------------------------------------------------------------------------------------------------
 // host-side objects
 // ------------------------------------------------------------------------------------------------
-static const uint32_t LANE_BYTES = 64;
-static const uint32_t WARP_BYTES = 32 * LANE_BYTES;          // 2 KiB per warp per tile
-static const uint32_t MAX_WARPS = 32;   // padding granularity (>= every variant's tile)
-static const uint32_t MAX_TILE = MAX_WARPS * WARP_BYTES;     // buffers are padded for the largest tile
+// scan_kernel's geometry: 16 warps of 32 lanes, each lane scanning 64 contiguous bytes of a 32 KiB tile (DESIGN §6 has the
+// measurement behind these values).  A tile is one TMA box of 128-byte rows.
+static const uint32_t SCAN_WARPS = 16;
+static const uint32_t SCAN_LANE_BYTES = 64;
+static const uint32_t SCAN_TILE = SCAN_WARPS * 32 * SCAN_LANE_BYTES;
+static const uint32_t SCAN_BOX_ROWS = SCAN_TILE / 128;
+static_assert(SCAN_BOX_ROWS <= 256, "a scan tile must fit one TMA box (at most 256 rows)");
+// padding granularity of a batch's buffer: the stream is followed by 0xFF up to a multiple of MAX_TILE plus one more MAX_TILE,
+// so the scan's last tile stays inside the allocation (other kernels may read into the padding too)
+static const uint32_t MAX_TILE = 64 * 1024;
+static_assert(MAX_TILE >= SCAN_TILE, "the padding must cover at least one scan tile");
 
 struct cf_ctx {
   int device = 0;
@@ -45,14 +52,7 @@ struct cf_ctx {
   std::vector<cudaEvent_t> prof_ev;
   uint32_t prof_used = 0;
   bool prof_on = false;
-  // scan kernel configuration (CF_SCAN_WARPS / CF_SCAN_ACC override the defaults; experiments)
-  uint32_t scan_warps = 16;        // defaults: see the CF_SCAN_* variables in include/cfgpu.h
-  uint32_t scan_lane_bytes = 64;
-  uint32_t scan_acc = 1;
-  uint32_t scan_stages = 3;
   uint32_t scan_reserve_sms = 0;   // CF_SCAN_RESERVE_SMS: SMs the persistent scan grid leaves free
-  uint32_t tile() const { return scan_warps * 32 * scan_lane_bytes; }
-  uint32_t box_rows() const { uint32_t rows = tile() / 128, nbox = (rows + 255) / 256; return rows / nbox; }
 };
 
 // the figures of an ordered rule that bound its output's growth (cf_sub_device's `worst`)

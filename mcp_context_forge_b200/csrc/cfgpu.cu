@@ -193,19 +193,17 @@ static const uint32_t WQ = 32;          // per-warp candidate staging slots in s
 static const uint32_t SCAN_SMEM = 227 * 1024;   // whole opt-in shared memory of the SM (1 CTA per SM)
 
 // Small per-CTA bookkeeping that lives next to the tile stages.
-static const uint32_t MAX_STAGES = 5;
-template <uint32_t WARPS>
+static const uint32_t MAX_STAGES = 5;   // mbarrier slots: at least the stages of either filter's ring
 struct ScanMisc {
-  alignas(8) unsigned long long wq[WARPS][WQ];
-  uint32_t wq_n[WARPS];
+  alignas(8) unsigned long long wq[SCAN_WARPS][WQ];
+  uint32_t wq_n[SCAN_WARPS];
   uint32_t cq_n;                   // candidates in this CTA's global queue segment
   alignas(8) uint64_t full[MAX_STAGES];
   alignas(8) uint64_t empty[MAX_STAGES];
 };
 
 // append one candidate (called by the few lanes that found one; divergent context)
-template <uint32_t WARPS>
-__device__ __noinline__ void push_candidate(ScanMisc<WARPS>& sm, const ScanParams& P, uint32_t warp, uint64_t pos) {
+__device__ __noinline__ void push_candidate(ScanMisc& sm, const ScanParams& P, uint32_t warp, uint64_t pos) {
   uint32_t slot = atomicAdd(&sm.wq_n[warp], 1u);
   if (slot < WQ) { sm.wq[warp][slot] = pos; return; }
   // staging full (pathologically dense candidates): go straight to the CTA queue
@@ -215,8 +213,7 @@ __device__ __noinline__ void push_candidate(ScanMisc<WARPS>& sm, const ScanParam
 }
 
 // warp-cooperative flush of the staging slots into the CTA's queue segment
-template <uint32_t WARPS>
-__device__ __forceinline__ void flush_candidates(ScanMisc<WARPS>& sm, const ScanParams& P, uint32_t warp, uint32_t lane) {
+__device__ __forceinline__ void flush_candidates(ScanMisc& sm, const ScanParams& P, uint32_t warp, uint32_t lane) {
   uint32_t n = sm.wq_n[warp];
   if (n > WQ) n = WQ;
   uint32_t base = 0;
@@ -250,11 +247,9 @@ __device__ __forceinline__ uint32_t lds_abs(uint32_t addr) {
   asm("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
   return v;
 }
-template <uint32_t ACC>
 __device__ __forceinline__ uint32_t pair_step(uint32_t acc, uint32_t f0, uint32_t e1, uint32_t mulc) {
   uint32_t t;
-  if (ACC == 1) asm("mad.lo.u32 %0, %1, %2, 1023;" : "=r"(t) : "r"(acc), "r"(mulc));
-  else t = (acc << 10) | 1023u;
+  asm("mad.lo.u32 %0, %1, %2, 1023;" : "=r"(t) : "r"(acc), "r"(mulc));
   return t & f0 & e1;
 }
 
@@ -263,11 +258,9 @@ __device__ __forceinline__ uint32_t pair_step(uint32_t acc, uint32_t f0, uint32_
   {                                                                                              \
     const uint32_t a0_ = __byte_perm((word), laneKF, 0x7604 | ((k) << 4));       /* F[b_k]   */  \
     const uint32_t a1_ = __byte_perm((word), laneK, 0x7604 | (((k) + 1) << 4));  /* E1[b_k+1] */ \
-    acc = pair_step<ACC>(acc, lds_abs(a0_), lds_abs(a1_), mulc);                                 \
+    acc = pair_step(acc, lds_abs(a0_), lds_abs(a1_), mulc);                                      \
     H |= acc;                                                                                    \
   }
-#define FEED4(word, H) FEEDP(word, 0, H) FEEDP(word, 2, H)
-#define FEED16(v, H) FEED4((v).x, H) FEED4((v).y, H) FEED4((v).z, H) FEED4((v).w, H)
 
 // rare path, lane-local: re-run one 16-byte group one byte at a time with position tracking
 // (data still in registers; E[b] is recovered from the E1 copy)
@@ -287,7 +280,7 @@ __device__ __forceinline__ uint32_t pair_step(uint32_t acc, uint32_t f0, uint32_
     while (m) {                                                                                 \
       const uint32_t k_ = __ffs(m) - 1;                                                         \
       m &= m - 1;                                                                               \
-      push_candidate<WARPS>(sm, P, warp, (gpos) + k_ - 3);                                      \
+      push_candidate(sm, P, warp, (gpos) + k_ - 3);                                             \
     }                                                                                           \
   }
 
@@ -330,20 +323,21 @@ __device__ __forceinline__ uint32_t pairq_step(uint32_t acc, uint32_t u, uint32_
     while (m_) {                                                      \
       const uint32_t k_ = __ffs(m_) - 1;                              \
       m_ &= m_ - 1;                                                   \
-      push_candidate<WARPS>(sm, P, warp, (gpos) + k_ - 3);            \
+      push_candidate(sm, P, warp, (gpos) + k_ - 3);                   \
     }                                                                 \
   }
 
-template <uint32_t WARPS, uint32_t LB, uint32_t ACC, uint32_t STAGES, uint32_t PAIR = 0>
-__global__ void __launch_bounds__(WARPS * 32, 1) scan_kernel(const __grid_constant__ ScanParams P,
-                                                               const __grid_constant__ CUtensorMap tmap) {
-  constexpr uint32_t NS = LB / 16;                  // 16-byte slots per lane per tile
-  constexpr uint32_t LPR = 128 / LB;                // lanes per 128-byte row
-  constexpr uint32_t TILE = WARPS * 32 * LB;
-  constexpr int32_t TROWS = TILE / 128;
-  constexpr int32_t NBOX = (TROWS + 255) / 256;     // TMA boxes per tile (box height <= 256 rows)
-  constexpr int32_t BROWS = TROWS / NBOX;
-  static_assert(BROWS * NBOX == TROWS, "tile rows must split evenly into TMA boxes");
+// PAIR = 0: byte prefilter; PAIR = 1: pair prefilter.  Geometry: SCAN_WARPS, SCAN_LANE_BYTES (cf_internal.h).
+template <uint32_t PAIR>
+__global__ void __launch_bounds__(SCAN_WARPS * 32, 1) scan_kernel(const __grid_constant__ ScanParams P,
+                                                                    const __grid_constant__ CUtensorMap tmap) {
+  // TMA ring depth: 3 for the byte filter (4 measured slower, DESIGN §6); the pair filter's 128 KiB table leaves room for 2
+  constexpr uint32_t STAGES = PAIR ? 2 : 3;
+  static_assert(STAGES <= MAX_STAGES, "one full / empty mbarrier pair per stage");
+  constexpr uint32_t NS = SCAN_LANE_BYTES / 16;     // 16-byte slots per lane per tile
+  static_assert(NS == 4, "the feeds below are written for 64 bytes per lane");
+  constexpr uint32_t LPR = 128 / SCAN_LANE_BYTES;   // lanes per 128-byte row
+  constexpr int32_t TROWS = SCAN_BOX_ROWS;          // a tile is one TMA box
   constexpr int32_t ROW0 = cf::FRONT_PAD / 128;     // stream byte 0 is row FRONT_PAD/128 of the buffer
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -357,16 +351,16 @@ __global__ void __launch_bounds__(WARPS * 32, 1) scan_kernel(const __grid_consta
   const uint32_t tbl_abs = PAIR ? ((abs0 + 1023u) & ~1023u) : ((abs0 + 0xFFFFu) & ~0xFFFFu);
   const uint32_t a_base = (abs0 + 1023u) & ~1023u;               // free space before the table
   const uint32_t b_base = tbl_abs + TBL_BYTES;                   // free space after it
-  const uint32_t na_fit = (tbl_abs - a_base) / TILE;
+  const uint32_t na_fit = (tbl_abs - a_base) / SCAN_TILE;
   const uint32_t NA = na_fit < STAGES ? na_fit : STAGES;
-  uint32_t a_end = a_base + NA * TILE, b_end = b_base + (STAGES - NA) * TILE;
+  uint32_t a_end = a_base + NA * SCAN_TILE, b_end = b_base + (STAGES - NA) * SCAN_TILE;
   uint32_t misc_abs;
-  if (a_end + sizeof(ScanMisc<WARPS>) <= tbl_abs) misc_abs = a_end; else { misc_abs = b_end; b_end += (uint32_t)sizeof(ScanMisc<WARPS>); }
-  if (b_end > abs0 + SCAN_SMEM) __trap();                        // cannot happen: variants are sized for 227 KiB
-  auto stage_abs = [&](uint32_t sidx) -> uint32_t { return sidx < NA ? a_base + sidx * TILE : b_base + (sidx - NA) * TILE; };
-  ScanMisc<WARPS>& sm = *reinterpret_cast<ScanMisc<WARPS>*>(smem_raw + (misc_abs - abs0));
-  const uint32_t full_abs = misc_abs + (uint32_t)offsetof(ScanMisc<WARPS>, full);
-  const uint32_t empty_abs = misc_abs + (uint32_t)offsetof(ScanMisc<WARPS>, empty);
+  if (a_end + sizeof(ScanMisc) <= tbl_abs) misc_abs = a_end; else { misc_abs = b_end; b_end += (uint32_t)sizeof(ScanMisc); }
+  if (b_end > abs0 + SCAN_SMEM) __trap();                        // cannot happen: both rings are sized for 227 KiB
+  auto stage_abs = [&](uint32_t sidx) -> uint32_t { return sidx < NA ? a_base + sidx * SCAN_TILE : b_base + (sidx - NA) * SCAN_TILE; };
+  ScanMisc& sm = *reinterpret_cast<ScanMisc*>(smem_raw + (misc_abs - abs0));
+  const uint32_t full_abs = misc_abs + (uint32_t)offsetof(ScanMisc, full);
+  const uint32_t empty_abs = misc_abs + (uint32_t)offsetof(ScanMisc, empty);
   uint32_t* tbl = reinterpret_cast<uint32_t*>(smem_raw + (tbl_abs - abs0));
   const uint32_t laneK = (lane << 2) | tbl_abs;                  // tbl_abs has zero low 16 bits
   const uint32_t laneKF = laneK | 0x80u;                         // second half of each row: the F copies
@@ -375,18 +369,16 @@ __global__ void __launch_bounds__(WARPS * 32, 1) scan_kernel(const __grid_consta
   (void)laneKF; (void)lane_base;
 
   auto load_tile = [&](uint32_t slot_, uint32_t tile_) {
-    mbar_expect_tx_a(full_abs + 8 * slot_, TILE);
-#pragma unroll
-    for (int32_t bx = 0; bx < NBOX; ++bx)
-      tma_load_2d_a(stage_abs(slot_) + bx * BROWS * 128, &tmap, 0, ROW0 + (int32_t)tile_ * TROWS + bx * BROWS, full_abs + 8 * slot_);
+    mbar_expect_tx_a(full_abs + 8 * slot_, SCAN_TILE);
+    tma_load_2d_a(stage_abs(slot_), &tmap, 0, ROW0 + (int32_t)tile_ * TROWS, full_abs + 8 * slot_);
   };
 
   const uint32_t first = blockIdx.x, stride = gridDim.x, ntiles = (uint32_t)P.ntiles;
-  if (tid < WARPS) sm.wq_n[tid] = 0;
+  if (tid < SCAN_WARPS) sm.wq_n[tid] = 0;
   if (tid == 0) {
     sm.cq_n = 0;
     if (blockIdx.x == 0) { P.qstate_next[0] = 0; P.qstate_next[1] = 0; }
-    for (uint32_t s = 0; s < STAGES; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], WARPS); }
+    for (uint32_t s = 0; s < STAGES; ++s) { mbar_init(&sm.full[s], 1); mbar_init(&sm.empty[s], SCAN_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     // prologue: put STAGES-1 tiles in flight right away; the table fill below overlaps their latency
     for (uint32_t j = 0; j < STAGES - 1; ++j) {
@@ -395,9 +387,9 @@ __global__ void __launch_bounds__(WARPS * 32, 1) scan_kernel(const __grid_consta
     }
   }
   if (PAIR) {
-    for (uint32_t i = tid; i < cf::PF_SLOTS * 32; i += WARPS * 32) tbl[i] = P.E[i >> 5];   // row h: 32 lane copies of T[h]
+    for (uint32_t i = tid; i < cf::PF_SLOTS * 32; i += SCAN_WARPS * 32) tbl[i] = P.E[i >> 5];   // row h: 32 lane copies of T[h]
   } else {
-    for (uint32_t i = tid; i < 256 * 32; i += WARPS * 32) {
+    for (uint32_t i = tid; i < 256 * 32; i += SCAN_WARPS * 32) {
       const uint32_t e = P.E[i >> 5];
       tbl[(i >> 5) * 64 + (i & 31)] = e | 0x3E000000u;            // E1
       tbl[(i >> 5) * 64 + 32 + (i & 31)] = (e << 5) | 31u;        // F
@@ -414,8 +406,8 @@ __global__ void __launch_bounds__(WARPS * 32, 1) scan_kernel(const __grid_consta
   const uint32_t ob = rowp * 128 + (((((gp % LPR) * NS) + NS - 1) ^ (rowp & 7)) << 4) + 12;
   // lane 0 of the CTA takes its look-back word (last 4 bytes of the previous tile) from HBM/L2,
   // fetched one iteration ahead
-  const uint8_t* back_ptr = P.stream + (uint64_t)first * TILE - 4;
-  const uint64_t back_step = (uint64_t)stride * TILE;
+  const uint8_t* back_ptr = P.stream + (uint64_t)first * SCAN_TILE - 4;
+  const uint64_t back_step = (uint64_t)stride * SCAN_TILE;
   uint32_t back_next = 0;
   if (tid == 0 && first < ntiles) back_next = *reinterpret_cast<const uint32_t*>(back_ptr);
 
@@ -438,8 +430,8 @@ __global__ void __launch_bounds__(WARPS * 32, 1) scan_kernel(const __grid_consta
     if (tid == 0 && t + stride < ntiles) back_next = *reinterpret_cast<const uint32_t*>(back_ptr);
     mbar_wait_a(full_abs + 8 * slot, phase);
 
-    // this lane's LB bytes (+ the word holding its 4 look-back bytes)
-    const uint32_t chunk = g * LB;          // tile-relative
+    // this lane's 64 bytes (+ the word holding its 4 look-back bytes)
+    const uint32_t chunk = g * SCAN_LANE_BYTES;   // tile-relative
     const uint32_t base = stage_abs(slot);
     if (g) back = lds32(base + ob);
     uint4 v[NS];
@@ -451,7 +443,6 @@ __global__ void __launch_bounds__(WARPS * 32, 1) scan_kernel(const __grid_consta
 
     uint32_t h[NS];
     if (PAIR) {
-      static_assert(!PAIR || NS == 4, "pair filter variant is written for 64 bytes per lane");
       // two independent chains (bytes 0-31 and 32-63), one byte per step
       uint32_t accA = 0, accB = 0;
       h[0] = h[1] = h[2] = h[3] = 0;
@@ -465,7 +456,7 @@ __global__ void __launch_bounds__(WARPS * 32, 1) scan_kernel(const __grid_consta
       QFEED4(accA, v[1].x, v[1].y, h[1]) QFEED4(accB, v[3].x, v[3].y, h[3])
       QFEED4(accA, v[1].y, v[1].z, h[1]) QFEED4(accB, v[3].y, v[3].z, h[3])
       QFEED4(accA, v[1].z, v[1].w, h[1]) QFEED4(accB, v[3].z, v[3].w, h[3])
-    } else if (NS == 4) {
+    } else {
       // two independent shift-AND chains per lane (bytes 0-31 and 32-63) for instruction-level
       // parallelism; the second chain re-feeds the last word of the first half as its look-back
       uint32_t accA = 0, accB = 0, dA = 0, dB = 0;
@@ -482,15 +473,6 @@ __global__ void __launch_bounds__(WARPS * 32, 1) scan_kernel(const __grid_consta
 #undef FEEDA
 #undef FEEDB
       (void)dA; (void)dB;
-    } else {
-      uint32_t acc = 0;
-      h[0] = 0;
-      FEED4(back, h[0])
-#pragma unroll
-      for (uint32_t j = 0; j < NS; ++j) {
-        h[j] = 0;   // (windows ending in the look-back bytes belong to the previous lane)
-        FEED16(v[j], h[j])
-      }
     }
 
     // rare path: an admissible 5-byte window ended in one of this lane's 16-byte groups
@@ -501,7 +483,7 @@ __global__ void __launch_bounds__(WARPS * 32, 1) scan_kernel(const __grid_consta
     const bool anyhit = (hany & HITM) != 0;
     if (__any_sync(0xFFFFFFFFu, anyhit)) {
       if (anyhit) {
-        const uint64_t cpos = (uint64_t)t * TILE + chunk;   // stream offset of this lane's first byte
+        const uint64_t cpos = (uint64_t)t * SCAN_TILE + chunk;   // stream offset of this lane's first byte
 #pragma unroll
         for (uint32_t j = 0; j < NS; ++j)
           if (h[j] & HITM) {
@@ -510,11 +492,11 @@ __global__ void __launch_bounds__(WARPS * 32, 1) scan_kernel(const __grid_consta
           }
       }
       __syncwarp();
-      if (sm.wq_n[warp] >= WQ / 2) flush_candidates<WARPS>(sm, P, warp, lane);
+      if (sm.wq_n[warp] >= WQ / 2) flush_candidates(sm, P, warp, lane);
     }
   }
   __syncwarp();
-  if (sm.wq_n[warp]) flush_candidates<WARPS>(sm, P, warp, lane);
+  if (sm.wq_n[warp]) flush_candidates(sm, P, warp, lane);
   __syncthreads();   // every tile this CTA requested has been consumed; table + tile buffers are free
 
   // ---- tail: verify this CTA's candidates, DFA tables staged over the (now idle) prefilter table
@@ -529,7 +511,7 @@ __global__ void __launch_bounds__(WARPS * 32, 1) scan_kernel(const __grid_consta
       const uint32_t words = (bytes + 3) / 4;
       const uint32_t* s32 = reinterpret_cast<const uint32_t*>(src);
       uint32_t* d32 = reinterpret_cast<uint32_t*>(dst + off_);
-      for (uint32_t i = tid; i < words; i += WARPS * 32) d32[i] = s32[i];
+      for (uint32_t i = tid; i < words; i += SCAN_WARPS * 32) d32[i] = s32[i];
       const void* r = dst + off_;
       off_ += (words * 4 + 15) & ~15u;
       return r;
@@ -544,31 +526,11 @@ __global__ void __launch_bounds__(WARPS * 32, 1) scan_kernel(const __grid_consta
   }
   uint32_t steps = 0;
   const unsigned long long* q = P.queue + (uint64_t)blockIdx.x * P.qcap_cta;
-  for (uint32_t i = lane * WARPS + warp; i < nq; i += WARPS * 32)   // spread over warps: less divergence
+  for (uint32_t i = lane * SCAN_WARPS + warp; i < nq; i += SCAN_WARPS * 32)   // spread over warps: less divergence
     verify_candidate(P, T, q[i], steps);
   for (int o = 16; o; o >>= 1) steps += __shfl_xor_sync(0xFFFFFFFFu, steps, o);
   if (lane == 0 && steps) atomicAdd(&P.qstate[1], (unsigned long long)steps);
   if (tid == 0) atomicAdd(&P.qstate[0], (unsigned long long)ncand);
-}
-
-typedef void (*scan_fn_t)(const ScanParams, const CUtensorMap);
-struct ScanVariant { scan_fn_t fn; uint32_t warps, lane_bytes, acc, stages; };
-// pair-filter kernels (128 KiB table): same tile geometry as the byte-filter variant in use, two stages
-static scan_fn_t pair_variant(uint32_t warps, uint32_t lane_bytes) {
-  if (warps == 16 && lane_bytes == 64) return scan_kernel<16, 64, 1, 2, 1>;
-  if (warps == 20 && lane_bytes == 64) return scan_kernel<20, 64, 1, 2, 1>;
-  return nullptr;
-}
-#define SV(W, LB, A, S) {scan_kernel<W, LB, A, S>, W, LB, A, S}
-static const ScanVariant SCAN_VARIANTS[] = {
-    SV(16, 64, 0, 3), SV(16, 64, 1, 3), SV(16, 64, 1, 4), SV(16, 64, 1, 2), SV(20, 64, 1, 3), SV(24, 64, 1, 3),
-    SV(16, 32, 1, 3), SV(24, 32, 1, 4), SV(32, 32, 1, 3), SV(32, 32, 1, 4),
-};
-#undef SV
-static const ScanVariant* scan_variant(uint32_t warps, uint32_t lane_bytes, uint32_t acc, uint32_t stages) {
-  for (const auto& v : SCAN_VARIANTS)
-    if (v.warps == warps && v.lane_bytes == lane_bytes && v.acc == acc && v.stages == stages) return &v;
-  return nullptr;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1025,16 +987,9 @@ int cf_init(int device_ordinal, cf_ctx** out) {
   CF_CUDA(ctx, cudaMalloc(&ctx->d_qstate, 4 * sizeof(uint64_t)));
   CF_CUDA(ctx, cudaMemset(ctx->d_qstate, 0, 4 * sizeof(uint64_t)));
   CF_CUDA(ctx, cudaMalloc(&ctx->d_queue, (size_t)ctx->qcap * sizeof(uint64_t)));
-  if (const char* e = getenv("CF_SCAN_WARPS")) ctx->scan_warps = (uint32_t)atoi(e);
-  if (const char* e = getenv("CF_SCAN_ACC")) ctx->scan_acc = (uint32_t)atoi(e);
-  if (const char* e = getenv("CF_SCAN_LB")) ctx->scan_lane_bytes = (uint32_t)atoi(e);
-  if (const char* e = getenv("CF_SCAN_STAGES")) ctx->scan_stages = (uint32_t)atoi(e);
   if (const char* e = getenv("CF_SCAN_RESERVE_SMS")) ctx->scan_reserve_sms = (uint32_t)atoi(e);
-  if (!scan_variant(ctx->scan_warps, ctx->scan_lane_bytes, ctx->scan_acc, ctx->scan_stages)) { ctx->err = "unsupported CF_SCAN_WARPS / CF_SCAN_LB / CF_SCAN_ACC / CF_SCAN_STAGES combination"; return CF_E_BADARG; }
-  for (const auto& v : SCAN_VARIANTS)
-    CF_CUDA(ctx, cudaFuncSetAttribute(v.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SCAN_SMEM));
-  if (scan_fn_t pf = pair_variant(ctx->scan_warps, ctx->scan_lane_bytes))
-    CF_CUDA(ctx, cudaFuncSetAttribute(pf, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SCAN_SMEM));
+  CF_CUDA(ctx, cudaFuncSetAttribute(scan_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SCAN_SMEM));
+  CF_CUDA(ctx, cudaFuncSetAttribute(scan_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SCAN_SMEM));
   return CF_OK;
 }
 
@@ -1070,7 +1025,7 @@ int cf_compile(cf_ctx* ctx, cf_builder* b, cf_prog** out) {
   p->W = b->out.search.W;
   *out = p;
   if ((rc = upload_dfa(ctx, b->out.search, p->search))) return rc;
-  p->use_pairs = b->out.filter.use_pairs && pair_variant(ctx->scan_warps, ctx->scan_lane_bytes) != nullptr;
+  p->use_pairs = b->out.filter.use_pairs;
   if (p->use_pairs) {   // large rule set: the pair prefilter's table instead of the byte table (scan_core.h)
     CF_CUDA(ctx, cudaMalloc(&p->d_E, cf::PF_SLOTS * 4));
     CF_CUDA(ctx, cudaMemcpy(p->d_E, b->out.filter.pairT.data(), cf::PF_SLOTS * 4, cudaMemcpyHostToDevice));
@@ -1172,7 +1127,7 @@ int cf_batch_create(cf_ctx* ctx, uint64_t max_stream_bytes, uint32_t max_units, 
   if (!fn || qres != cudaDriverEntryPointSuccess) { ctx->err = "cuTensorMapEncodeTiled unavailable"; return CF_E_CUDA; }
   cuuint64_t gdim[2] = {128, total / 128};
   cuuint64_t gstride[1] = {128};
-  cuuint32_t box[2] = {128, ctx->box_rows()};
+  cuuint32_t box[2] = {128, SCAN_BOX_ROWS};
   cuuint32_t estr[2] = {1, 1};
   CUresult cr = ((encode_fn)fn)(&b->tmap, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, b->d_buf, gdim, gstride, box, estr,
                                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
@@ -1244,8 +1199,7 @@ int cf_scan(cf_ctx* ctx, cf_prog* p, cf_batch* b, uint64_t* d_bitmaps, void* cud
 }  // extern "C"
 
 int cf_scan_launch(cf_ctx* ctx, cf_prog* p, cf_batch* b, uint64_t* d_bitmaps, cudaStream_t st, uint64_t* queue, uint64_t* qstate, uint32_t* qphase) {
-  const uint32_t tile = ctx->tile();
-  const uint64_t ntiles = ntiles_for(b->nbytes, tile);
+  const uint64_t ntiles = ntiles_for(b->nbytes, SCAN_TILE);
   const uint64_t total = (uint64_t)b->n * p->W;
   if (p->any_always) {
     fill_bitmaps_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(d_bitmaps, p->d_always, p->W, total);
@@ -1274,14 +1228,13 @@ int cf_scan_launch(cf_ctx* ctx, cf_prog* p, cf_batch* b, uint64_t* d_bitmaps, cu
   P.dfa_trans_bytes = (uint32_t)p->search.trans_bytes;
   P.dfa_acc_bytes = (uint32_t)p->search.acc_bytes;
   P.mulc = p->use_pairs ? 256 : 1024;
-  const ScanVariant* sv = scan_variant(ctx->scan_warps, ctx->scan_lane_bytes, ctx->scan_acc, ctx->scan_stages);
-  const scan_fn_t fn = p->use_pairs ? pair_variant(ctx->scan_warps, ctx->scan_lane_bytes) : sv->fn;
+  const auto fn = p->use_pairs ? scan_kernel<1> : scan_kernel<0>;
   uint64_t grid = (uint64_t)ctx->sm_count;   // persistent: one CTA per SM
   if (ctx->scan_reserve_sms && ctx->scan_reserve_sms < grid) grid -= ctx->scan_reserve_sms;
   if (grid > ntiles) grid = ntiles;
   const bool prof = ctx->prof_on && (size_t)ctx->prof_used + 2 <= ctx->prof_ev.size();
   if (prof) cudaEventRecord(ctx->prof_ev[ctx->prof_used], st);
-  fn<<<(unsigned)grid, sv->warps * 32, SCAN_SMEM, st>>>(P, b->tmap);
+  fn<<<(unsigned)grid, SCAN_WARPS * 32, SCAN_SMEM, st>>>(P, b->tmap);
   if (prof) { cudaEventRecord(ctx->prof_ev[ctx->prof_used + 1], st); ctx->prof_used += 2; }
   ctx->launches++;
   CF_CUDA(ctx, cudaGetLastError());

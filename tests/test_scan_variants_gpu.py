@@ -1,18 +1,19 @@
-"""Every compiled scan-kernel variant against the oracle (CPython `re` / `in`), at the places where a persistent TMA-ring
-scan goes wrong: a match exactly on a tile edge, on the stage-ring wrap and on lane-chunk edges, with a multi-byte
+"""Both scan kernels (byte and pair prefilter) against the oracle (CPython `re` / `in`), at the places where a persistent
+TMA-ring scan goes wrong: a match exactly on a tile edge, on the stage-ring wrap and on lane-chunk edges, with a multi-byte
 character or a unit terminator right in front of it; a candidate-dense stream that overflows the candidate queue; bitmaps
 of 1, 2 and 4 words; an always-matching pattern; random patterns.
 
-The library reads CF_SCAN_* once, in cf_init, and a Context is cached per process, so each configuration runs in a worker
-process of its own (this file, `--worker`).  The parent writes the corpora, runs the worker with the configuration's
+The library reads CF_SCAN_RESERVE_SMS once, in cf_init, and a Context is cached per process, so each configuration runs in a
+worker process of its own (this file, `--worker`).  The parent writes the corpora, runs the worker with the configuration's
 environment, and compares the bitmaps the worker saved with the oracle, which it computes once per corpus.
 
-The variant list below must equal SCAN_VARIANTS and pair_variant in csrc/cfgpu.cu (checked without a GPU), so a new
-variant cannot go untested."""
+The geometry below must equal the kernels' (checked without a GPU), so that the planted matches land on their real tile,
+lane and stage-ring edges."""
 import json
 import os
 import random
 import re
+import shutil
 import subprocess
 import sys
 
@@ -24,15 +25,16 @@ for _p in (ROOT, os.path.join(ROOT, "tests")):
     if _p not in sys.path:
         sys.path.insert(0, _p)
 
-from mcp_context_forge_b200 import engine  # noqa: E402
+from mcp_context_forge_b200 import _native, engine  # noqa: E402
 from oracle import hook_chain_ref as ref  # noqa: E402
 
-CFGPU = os.path.join(ROOT, "mcp_context_forge_b200", "csrc", "cfgpu.cu")
+CSRC = os.path.join(ROOT, "mcp_context_forge_b200", "csrc")
 
-# (warps, lane bytes, acc, stages) of scan_kernel's byte-filter variants, and (warps, lane bytes) of its pair-filter ones
-BYTE_VARIANTS = [(16, 64, 0, 3), (16, 64, 1, 3), (16, 64, 1, 4), (16, 64, 1, 2), (20, 64, 1, 3), (24, 64, 1, 3),
-                 (16, 32, 1, 3), (24, 32, 1, 4), (32, 32, 1, 3), (32, 32, 1, 4)]
-PAIR_VARIANTS = [(16, 64), (20, 64)]
+# scan_kernel's geometry (csrc/cf_internal.h) and the depth of its TMA stage ring per prefilter (csrc/cfgpu.cu)
+WARPS = 16
+LANE_BYTES = 64
+TILE = WARPS * 32 * LANE_BYTES
+BYTE_STAGES = 3
 PAIR_STAGES = 2
 
 HARMFUL = [(p, re.I) for pats in ref.DEFAULT_LEXICONS.values() for p in pats]
@@ -64,7 +66,7 @@ TAIL = " ok."
 FILL = ("lorem ipsum dolor sit amet, consectetur adipiscing elit; sed do eiusmod tempor incididunt ut labore et dolore "
         "magna aliqua. ") * 8
 EDGE_DS = list(range(-12, 5))                         # match start = edge + d
-EDGE_TILES = 5                                        # tile edges 1..5: the first three, and (with one CTA) the ring wrap of 2, 3 and 4 stages
+EDGE_TILES = 5                                        # tile edges 1..5: the first three, and (with one CTA) the ring wrap of 2 and 3 stages
 
 
 def filler(n):
@@ -159,26 +161,19 @@ def fuzz_round(seed):
     return pats, units
 
 
-def geometry(cfg):
-    """(tile bytes, lane bytes) of a configuration's kernel."""
-    w, lb = cfg["warps"], cfg["lb"]
-    return w * 32 * lb, lb
-
-
 def configurations(sms=132):
-    """Every variant on the full persistent grid (all corpora), and again with one CTA (edge corpus only).  On the full grid
-    an edge stream of a few tiles gives each CTA one tile, so its stage ring never wraps; with one CTA, tile k sits in stage
-    k mod stages and the planted edges k = 1..5 cross the ring wrap of 2, 3 and 4 stages."""
+    """Each prefilter's kernel on the full persistent grid (all corpora), and again with one CTA (edge corpus only).  On the
+    full grid an edge stream of a few tiles gives each CTA one tile, so its stage ring never wraps; with one CTA, tile k sits
+    in stage k mod stages and the planted edges k = 1..5 cross the ring wrap of the byte filter's 3 stages and the pair
+    filter's 2."""
     cfgs = []
-    variants = [(f"byte-{w}w-{lb}lb-acc{acc}-{st}st", w, lb, False, {"CF_SCAN_WARPS": w, "CF_SCAN_LB": lb, "CF_SCAN_ACC": acc, "CF_SCAN_STAGES": st, "CF_PAIR_FILTER": 0})
-                for w, lb, acc, st in BYTE_VARIANTS]
-    variants += [(f"pair-{w}w-{lb}lb", w, lb, True, {"CF_SCAN_WARPS": w, "CF_SCAN_LB": lb, "CF_PAIR_FILTER": 1}) for w, lb in PAIR_VARIANTS]
-    for name, w, lb, pair, env in variants:
-        cfgs.append({"id": name, "warps": w, "lb": lb, "pair": pair, "edge_only": False, "env": env})
-        cfgs.append({"id": name + "-one-cta", "warps": w, "lb": lb, "pair": pair, "edge_only": True, "env": dict(env, CF_SCAN_RESERVE_SMS=sms - 1)})
-    cfgs.append({"id": "default-reserve-4", "warps": 16, "lb": 64, "pair": False, "edge_only": False, "env": {"CF_SCAN_RESERVE_SMS": 4, "CF_PAIR_FILTER": 0}})
+    for name, pair in (("byte", False), ("pair", True)):
+        env = {"CF_PAIR_FILTER": int(pair)}
+        cfgs.append({"id": name, "pair": pair, "edge_only": False, "env": env})
+        cfgs.append({"id": name + "-one-cta", "pair": pair, "edge_only": True, "env": dict(env, CF_SCAN_RESERVE_SMS=sms - 1)})
+    cfgs.append({"id": "default-reserve-4", "pair": False, "edge_only": False, "env": {"CF_SCAN_RESERVE_SMS": 4, "CF_PAIR_FILTER": 0}})
     # one CTA owns every tile of the candidate-dense corpus: its share of the candidate queue overflows
-    cfgs.append({"id": "default-one-cta", "warps": 16, "lb": 64, "pair": False, "edge_only": False, "env": {"CF_SCAN_RESERVE_SMS": sms - 1, "CF_PAIR_FILTER": 0}})
+    cfgs.append({"id": "default-one-cta", "pair": False, "edge_only": False, "env": {"CF_SCAN_RESERVE_SMS": sms - 1, "CF_PAIR_FILTER": 0}})
     return cfgs
 
 
@@ -188,26 +183,24 @@ CONFIG_IDS = [c["id"] for c in configurations()]
 # ---------------------------------------------------------------------------------------------------------------------
 # CPU checks
 # ---------------------------------------------------------------------------------------------------------------------
-def test_variant_list_matches_the_library_source():
-    src = open(CFGPU, encoding="utf-8").read()
-    block = src[src.index("static const ScanVariant SCAN_VARIANTS[]"):]
-    block = block[:block.index("};")]
-    byte = [tuple(int(x) for x in m) for m in re.findall(r"SV\((\d+),\s*(\d+),\s*(\d+),\s*(\d+)\)", block)]
-    assert sorted(byte) == sorted(BYTE_VARIANTS)
-    fn = src[src.index("static scan_fn_t pair_variant"):]
-    fn = fn[:fn.index("\n}")]
-    pair = re.findall(r"warps == (\d+) && lane_bytes == (\d+)\) return scan_kernel<(\d+), (\d+), 1, (\d+), 1>", fn)
-    assert pair and all(a == c and b == d and int(s) == PAIR_STAGES for a, b, c, d, s in pair)
-    assert sorted((int(a), int(b)) for a, b, _, _, _ in pair) == sorted(PAIR_VARIANTS)
-    # the defaults of cf_ctx are one of the byte variants
-    hdr = open(os.path.join(ROOT, "mcp_context_forge_b200", "csrc", "cf_internal.h"), encoding="utf-8").read()
-    dflt = tuple(int(re.search(rf"uint32_t {k} = (\d+);", hdr).group(1)) for k in ("scan_warps", "scan_lane_bytes", "scan_acc", "scan_stages"))
-    assert dflt in BYTE_VARIANTS
+def test_geometry_matches_the_library():
+    """The corpora's geometry is the kernels' (read from the source), and the built library holds exactly the two kernels."""
+    hdr = open(os.path.join(CSRC, "cf_internal.h"), encoding="utf-8").read()
+    assert int(re.search(r"uint32_t SCAN_WARPS = (\d+);", hdr).group(1)) == WARPS
+    assert int(re.search(r"uint32_t SCAN_LANE_BYTES = (\d+);", hdr).group(1)) == LANE_BYTES
+    src = open(os.path.join(CSRC, "cfgpu.cu"), encoding="utf-8").read()
+    pair_st, byte_st = re.search(r"constexpr uint32_t STAGES = PAIR \? (\d+) : (\d+);", src).groups()
+    assert (int(byte_st), int(pair_st)) == (BYTE_STAGES, PAIR_STAGES)
+    cuobjdump = next((c for c in (shutil.which("cuobjdump"), "/usr/local/cuda/bin/cuobjdump") if c and os.path.exists(c)), None)
+    if cuobjdump is None:
+        pytest.skip("cuobjdump not found")
+    out = subprocess.run([cuobjdump, "--dump-resource-usage", _native.SO_PATH], capture_output=True, text=True, check=True).stdout
+    kernels = sorted(set(re.findall(r"Function (\S*scan_kernel\S*):", out)))
+    assert kernels == ["_Z11scan_kernelILj0EEv10ScanParams14CUtensorMap_st", "_Z11scan_kernelILj1EEv10ScanParams14CUtensorMap_st"], kernels
 
 
-@pytest.mark.parametrize("geom", sorted({geometry(c) for c in configurations()}), ids=lambda g: f"{g[0]}B-tile-{g[1]}B-lanes")
-def test_edge_corpus_places_every_match_where_intended(geom):
-    tile, lb = geom
+def test_edge_corpus_places_every_match_where_intended():
+    tile, lb = TILE, LANE_BYTES
     seen = set()
     for d, (units, placements) in zip(EDGE_DS, edge_corpus(tile, lb)):
         stream, offs = engine.pack_units(units)
@@ -262,10 +255,9 @@ class Corpora:
 
     def jobs(self, cfg):
         """[(program spec, corpus key, corpus path, oracle function)] for one configuration."""
-        tile, lb = geometry(cfg)
         out = []
-        for i, (units, _) in enumerate(edge_corpus(tile, lb)):
-            key = f"edge-{tile}-{lb}-{i}"
+        for i, (units, _) in enumerate(edge_corpus(TILE, LANE_BYTES)):
+            key = f"edge-{i}"
             path = self._write(key, units)
             for prog in PROGRAMS:
                 out.append((prog, key, path, lambda u, p=prog: _oracle(p, u)))
@@ -297,7 +289,7 @@ def _run_worker(job, env_over, tmp_path, timeout=600):
     with open(jf, "w") as f:
         json.dump(job, f)
     env = dict(os.environ)
-    for k in ("CF_SCAN_WARPS", "CF_SCAN_LB", "CF_SCAN_ACC", "CF_SCAN_STAGES", "CF_SCAN_RESERVE_SMS", "CF_PAIR_FILTER"):
+    for k in ("CF_SCAN_RESERVE_SMS", "CF_PAIR_FILTER"):
         env.pop(k, None)
     env.update({k: str(v) for k, v in env_over.items()})
     r = subprocess.run([sys.executable, os.path.abspath(__file__), "--worker", jf], env=env, cwd=ROOT, capture_output=True, text=True, timeout=timeout)
@@ -334,13 +326,6 @@ def test_variant_matches_oracle(idx, corpora, tmp_path):
     assert checked > 1000
     if cfg["id"] == "default-one-cta":
         assert res["dense_candidates"] > (1 << 20)        # far more than one CTA's share of the candidate queue
-
-
-@pytest.mark.gpu
-def test_unsupported_variant_is_refused(tmp_path):
-    """CF_SCAN_WARPS=17 names no compiled variant: Context() raises (which also shows that the workers see their environment)."""
-    res = _run_worker({"out": str(tmp_path), "scans": []}, {"CF_SCAN_WARPS": 17}, tmp_path, timeout=120)
-    assert res["error"] and "unsupported CF_SCAN_WARPS" in res["error"], res
 
 
 # ---------------------------------------------------------------------------------------------------------------------
