@@ -390,6 +390,23 @@ int cf_chain(cf_ctx* ctx, cf_prog* prog, cf_batch* b, uint32_t stage_mask, uint3
   return CF_OK;
 }
 
+#ifdef CF_TOON_PHASES
+// Phase-timing builds only (json_tp.h TP_PHASE): out[k] = the cycles all warps spent in phase k since the last call, which clears them.
+int cf_toon_phase_cycles(unsigned long long* out) {
+  const size_t n = (size_t)cftp::PH_WARPS * (cftp::PH_N + 1);
+  unsigned long long* h = (unsigned long long*)calloc(n, sizeof(unsigned long long));
+  if (!h) return CF_E_NOMEM;
+  cudaError_t e = cudaMemcpyFromSymbol(h, cftp::toon_phase_cycles, n * sizeof(unsigned long long));
+  for (uint32_t k = 0; k < cftp::PH_N; ++k) out[k] = 0;
+  for (size_t w = 0; w < cftp::PH_WARPS; ++w)
+    for (uint32_t k = 0; k < cftp::PH_N; ++k) out[k] += h[w * (cftp::PH_N + 1) + k];
+  memset(h, 0, n * sizeof(unsigned long long));
+  if (e == cudaSuccess) e = cudaMemcpyToSymbol(cftp::toon_phase_cycles, h, n * sizeof(unsigned long long));
+  free(h);
+  return e == cudaSuccess ? CF_OK : CF_E_CUDA;
+}
+#endif
+
 // Not part of the C API (include/cfgpu.h): the token-parallel kernel's launch shape for tests/test_toon_occupancy_cpu.py, which
 // checks it against the built kernel's resource usage without a device.
 void cf_toon_tp_config(uint32_t* warps_per_cta, uint32_t* ctas_per_sm, uint32_t* smem_per_cta) {

@@ -40,6 +40,25 @@ using cfj::TS_VALUE_ERROR;
 enum : int { TS_FALLBACK = 7 };      // internal: bits 8.. carry the reason (FB_*), stripped at the ABI
 enum : uint32_t { FB_NUM_EXACT = 1, FB_KEY_ESCAPE = 2, FB_TOK_CAP = 3, FB_KH_CAP = 4, FB_DUP_HASH = 5, FB_ROW_ORDER = 6, FB_MIXED_ITEM = 7, FB_TOO_LONG = 8 };
 
+// ---- phase timing: build option CF_TOON_PHASES, off in the shipped library (tools/toon_phase_breakdown.py builds it) ----
+// Lane 0 of each warp adds the clock64() cycles of each phase to the warp's row of toon_phase_cycles (warp slots wrap around at
+// PH_WARPS).  Column PH_N is the warp's "inside the resolve retry" flag: the retry's cycles count once, in PH_RESOLVE.
+enum : uint32_t { PH_TOKENIZE = 0, PH_AN_GENERIC = 1, PH_AN_TABLE = 2, PH_EM_GENERIC = 3, PH_EM_TABLE = 4, PH_RESOLVE = 5, PH_N = 6 };
+#if defined(CF_TOON_PHASES) && defined(__CUDACC__)
+static const uint32_t PH_WARPS = 1u << 16;
+__device__ unsigned long long toon_phase_cycles[PH_WARPS * (PH_N + 1)];
+TP_FN unsigned long long* ph_row() { return toon_phase_cycles + ((blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) % PH_WARPS) * (PH_N + 1); }
+TP_FN void ph_add(uint32_t k, unsigned long long t0) {
+  const unsigned long long t1 = clock64();
+  if (tpw::lane() == 0 && (k == PH_RESOLVE || !ph_row()[PH_N])) atomicAdd(ph_row() + k, t1 - t0);
+}
+TP_FN void ph_in_retry(bool on) { if (tpw::lane() == 0) ph_row()[PH_N] = on ? 1ull : 0ull; }
+#define TP_PHASE(k, ...) do { const unsigned long long ph_t0_ = clock64(); __VA_ARGS__; ph_add((k), ph_t0_); } while (0)
+#else
+TP_FN void ph_in_retry(bool) {}
+#define TP_PHASE(k, ...) do { __VA_ARGS__; } while (0)
+#endif
+
 // ---- tokens --------------------------------------------------------------------------------------------------------
 enum : uint32_t { K_OPEN_OBJ = 0, K_OPEN_ARR = 1, K_CLOSE_OBJ = 2, K_CLOSE_ARR = 3, K_STR = 4, K_KEY = 5, K_NUM = 6, K_LIT = 7 };
 struct GTok { uint32_t pos, w; };                 // w = kind:3 | flags:5 | commas:2 | colons:2 | len:20
@@ -1072,13 +1091,15 @@ TP_FN int analyze(const uint8_t* s, GTok* toks, uint32_t ntok, uint32_t tok_cap,
     if (!force && st.sp > 0 && table_candidate(sh, st.sp - 1) && gt_kind(toks[i].w) == K_OPEN_OBJ) {
       const uint32_t S = 2 + 2 * sh.row0_n[st.sp - 1];
       bool staged_only;
-      const uint32_t g = an_rows(s, toks, ntok, sh, stage, st, i, &staged_only);
+      uint32_t g;
+      TP_PHASE(PH_AN_TABLE, g = an_rows(s, toks, ntok, sh, stage, st, i, &staged_only));
       i += g * S;
       if (g < 32 && !staged_only) force = true;       // the next row (if it is one) does not conform: generic walk
       continue;
     }
     const uint32_t m = ntok - i > 32 ? 32u : ntok - i;
-    const uint32_t c = an_batch<RESOLVE_MIXED>(s, toks, tok_cap, sh, st, i, m, force);
+    uint32_t c;
+    TP_PHASE(PH_AN_GENERIC, c = an_batch<RESOLVE_MIXED>(s, toks, tok_cap, sh, st, i, m, force));
     force = false;
     i += c;
   }
@@ -1126,6 +1147,8 @@ TP_FN void cell_put(Emit& em, const uint8_t* s, const GTok t) {
   em.span(s + t.pos, len);
   if (q) em.put('"');
 }
+
+static const uint32_t SPAN_LOADS = 8;     // long spans (em_batch): bytes each lane loads before it stores them
 
 // Generic mode: tokens [i, i+m).  Returns the number consumed: the batch ends right behind the header of a table.
 TP_FN uint32_t em_batch(const uint8_t* s, const GTok* toks, uint32_t ntok, uint8_t* out, uint32_t out_cap, Shared& sh, EmState& st, uint32_t i, uint32_t m,
@@ -1315,7 +1338,15 @@ TP_FN uint32_t em_batch(const uint8_t* s, const GTok* toks, uint32_t ntok, uint8
     lm &= lm - 1;
     const uint32_t jpos = tpw::shfl(t.pos, j), jlen = tpw::shfl(len, j);
     const uint32_t jdst = tpw::shfl(off + plen - blen + (pc.body == B_QSPAN ? 1u : 0u), j);
-    for (uint32_t k = l; k < jlen; k += 32) if (jdst + k < out_cap) out[jdst + k] = s[jpos + k];
+    // SPAN_LOADS bytes per lane per round, every load issued before the round's stores: `out` may alias `s` as far as the compiler
+    // knows, so a load behind a store waits for it, and one byte per round paid a full L2 round trip per 32 bytes of a long string
+    for (uint32_t b = 0; b < jlen; b += 32 * SPAN_LOADS) {
+      uint8_t v[SPAN_LOADS];
+#pragma unroll
+      for (uint32_t q = 0; q < SPAN_LOADS; ++q) { const uint32_t k = b + 32 * q + l; v[q] = k < jlen ? s[jpos + k] : (uint8_t)0; }
+#pragma unroll
+      for (uint32_t q = 0; q < SPAN_LOADS; ++q) { const uint32_t k = b + 32 * q + l; if (k < jlen && jdst + k < out_cap) out[jdst + k] = v[q]; }
+    }
   }
   st.ocur += total;
   return consumed;
@@ -1385,9 +1416,9 @@ TP_FN int emit(const uint8_t* s, const GTok* toks, uint32_t ntok, uint8_t* out, 
   uint32_t i = 0;
   while (i < ntok && !st.status) {
     const uint32_t m = ntok - i > 32 ? 32u : ntok - i;
-    i += em_batch(s, toks, ntok, out, out_cap, sh, st, i, m, report_errors);
+    TP_PHASE(PH_EM_GENERIC, i += em_batch(s, toks, ntok, out, out_cap, sh, st, i, m, report_errors));
     if (!st.status && st.col_rows) {
-      em_rows(s, toks, out, out_cap, sh, stage, st, report_errors);
+      TP_PHASE(PH_EM_TABLE, em_rows(s, toks, out, out_cap, sh, stage, st, report_errors));
       i = st.col_first + st.col_rows * (2 + 2 * st.col_rn);       // the table's closing bracket comes next
     }
   }
@@ -1430,13 +1461,16 @@ TP_SLOW int toon_tokens_resolve(const uint8_t* s, GTok* toks, uint32_t ntok, uin
 TP_FN int toon_unit(const uint8_t* s, uint32_t n, GTok* toks, uint32_t tok_cap, uint8_t* out, uint32_t out_cap, uint32_t* out_len, Shared& sh,
                     uint8_t* stage, bool report_errors, bool retry_mixed = false) {
   uint32_t ntok = 0;
-  int st = tokenize(s, n, toks, tok_cap, sh, stage, &ntok);
+  int st;
+  TP_PHASE(PH_TOKENIZE, st = tokenize(s, n, toks, tok_cap, sh, stage, &ntok));
   if (st) return st;
   tpw::sync();
   st = toon_tokens<false>(s, toks, ntok, tok_cap, out, out_cap, out_len, sh, stage, report_errors);
   if (retry_mixed && st == (TS_FALLBACK | (int)(FB_MIXED_ITEM << 8))) {
     tpw::sync();
-    st = toon_tokens_resolve(s, toks, ntok, tok_cap, out, out_cap, out_len, sh, stage, report_errors);
+    ph_in_retry(true);
+    TP_PHASE(PH_RESOLVE, st = toon_tokens_resolve(s, toks, ntok, tok_cap, out, out_cap, out_len, sh, stage, report_errors));
+    ph_in_retry(false);
   }
   return st;
 }
