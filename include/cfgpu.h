@@ -26,7 +26,7 @@
  *          what `orjson.loads` (toon_encoder.py:281), `serde_json::from_slice` (lib.rs:353) and the
  *          string walk `_iter_strings` (harmful_content_detector.py:110-139) each recompute per payload
  *
- *   cf_run_batch / cf_chain / cf_run_enqueue + cf_run_finish
+ *   cf_run_batch / cf_run_enqueue + cf_run_finish
  *       -> the whole per-request plugin chain over one uploaded batch (mcpgateway/services/tool_service.py:5866-5872)
  *
  * Environment (read once per process):
@@ -98,7 +98,7 @@ int cf_builder_compile_host(cf_builder* b, cf_compile_stats* out);
  * stream's work: calls on ONE cf_ctx must be serialised by the caller (the Python binding holds a lock per context; a gateway
  * worker has one context and one launching thread).  Different cf_ctx objects — one per worker process or per GPU — are
  * independent.  A compiled cf_prog is immutable and may be used by any call of the ctx that compiled it; a cf_batch holds ONE
- * upload at a time.  The asynchronous entry points (cf_scan, cf_toon, cf_chain, cf_run_enqueue) only enqueue on the given stream and
+ * upload at a time.  The asynchronous entry points (cf_scan, cf_toon, cf_run_enqueue) only enqueue on the given stream and
  * return. */
 int cf_init(int device_ordinal, cf_ctx** out);
 void cf_shutdown(cf_ctx* ctx);
@@ -209,7 +209,8 @@ int cf_toon_host(cf_ctx* ctx, cf_batch* b, uint32_t flags, const uint8_t* stream
  * stream == NULL runs the stages on the batch that is ALREADY resident (uploaded by cf_batch_upload or a previous call): bench.py's
  * device-resident `value`; offsets must then be the host copy of that batch's offsets.
  *   CF_STAGE_MASK  request_logging_masking on the same upload (verdict.aux = CF_MASK_* status, out = masked JSON);
- *                  not combinable with CF_STAGE_TOON in one call (both produce the unit's output). */
+ *                  not combinable with CF_STAGE_TOON in one call (both produce the unit's output).  Rewritten texts are not
+ *                  returned: a rewritten unit that does not mask keeps its rewritten length in out_len and has no output. */
 #define CF_STAGE_SCAN 1u
 #define CF_STAGE_SUB 2u
 #define CF_STAGE_MASK 4u
@@ -237,21 +238,18 @@ int cf_run_batch(cf_ctx* ctx, cf_prog* prog /* may be NULL without SCAN/SUB */, 
 int cf_run_batch_device_output(cf_ctx* ctx, const uint8_t** d_out, uint64_t* bytes);
 /* synchronous copy of `bytes` device bytes to a host buffer (for callers without a CUDA runtime binding of their own) */
 int cf_copy_to_host(cf_ctx* ctx, void* host_dst, const void* device_src, uint64_t bytes);
-/* device-resident, asynchronous on cuda_stream: CF_STAGE_SCAN and/or CF_STAGE_TOON over the batch already uploaded (what
- * bench.py times with the batch resident in HBM).  d_unit_stages may be NULL. */
-int cf_chain(cf_ctx* ctx, cf_prog* prog, cf_batch* b, uint32_t stage_mask, uint32_t toon_flags, uint64_t* d_bitmaps, const uint8_t* d_unit_stages,
-             uint8_t* d_out, uint32_t* d_out_len, int32_t* d_status, void* cuda_stream);
 
 /* ---------------- the fused chain on the caller's stream: cf_run_enqueue / cf_run_finish ----------------
  * cf_run_batch's SCAN, SUB and TOON stages without a host round trip between launch and completion: the dirty-unit selection, the
  * substitution's scratch bounds and arena allocation, the verdict records, the output offsets and the gather are decided on the
- * device.  cf_run_batch itself (without CF_STAGE_MASK) is an upload, one enqueue and one finish on a run the context owns.
+ * device.  cf_run_batch itself is an upload, one enqueue and one finish on a run the context owns (with CF_STAGE_MASK, the masking
+ * kernel after them).
  *
  * A cf_run owns every piece of per-call device state (scan queue, TOON scratch and unit order, the dirty-unit list, the substitution
  * descriptors and arena, per-unit gather sources, a status block, a completion event and a side stream), so runs created on one
  * ctx can be in flight at once on different streams.  Memory of a run: 8 x max_stream_bytes of TOON scratch, max_stream_bytes of
  * TOON output, about 170 bytes per unit, 8 MiB of scan queue and the arena.  (The run cf_run_batch uses borrows the context's TOON
- * workspace instead, the one cf_toon and cf_chain use, so a context holds one.)
+ * workspace instead, the one cf_toon uses, so a context holds one.)
  *
  * cf_run_enqueue: the batch must be resident (cf_batch_upload on the same stream, or ordered before it).  d_verdicts (n_units
  * records), d_out_offsets (n_units + 1), d_out (out_cap bytes), d_bitmaps_full (n_units * W words; required with SCAN or SUB) and
@@ -290,8 +288,8 @@ int cf_profile_collect(cf_ctx* ctx, double* total_ms, uint32_t* n_launches);
 /* same, one duration per recorded launch, in launch order (cf_scan and the TOON stage record one pair each); resets the list */
 int cf_profile_collect_each(cf_ctx* ctx, double* ms, uint32_t cap, uint32_t* n_launches);
 
-/* device-side counters of the last cf_scan / cf_scan_host / CF_STAGE_MASK cf_run_batch scan: [0]=prefilter candidates, [1]=DFA verify
- * steps.  cf_run_enqueue (and cf_run_batch without CF_STAGE_MASK, which runs through it) counts on its run's own pair. */
+/* device-side counters of the last cf_scan / cf_scan_host scan: [0]=prefilter candidates, [1]=DFA verify steps.  cf_run_enqueue
+ * (and cf_run_batch, which runs through it) counts on its run's own pair. */
 int cf_scan_counters(cf_ctx* ctx, uint64_t out[2]);
 
 #ifdef __cplusplus

@@ -64,7 +64,6 @@ _SIGS = {
     "cf_json_index_host": (c_int, [c_void_p, c_void_p, c_uint32, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_void_p]),
     "cf_run_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_uint32, c_void_p, c_uint32, c_int, c_void_p, c_void_p,
                              c_void_p, c_uint64, c_void_p, POINTER(c_uint64)]),
-    "cf_chain": (c_int, [c_void_p, c_void_p, c_void_p, c_uint32, c_uint32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "cf_run_create": (c_int, [c_void_p, c_uint32, c_uint64, c_uint64, POINTER(c_void_p)]),
     "cf_run_free": (None, [c_void_p]),
     "cf_run_enqueue": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_uint32, c_void_p, c_void_p, c_void_p, c_void_p, c_uint64,

@@ -264,7 +264,7 @@ int cf_json_index_host(cf_ctx* ctx, cf_batch* b, uint32_t flags, const uint8_t* 
 }
 
 // TOON device workspace: token / DOM scratch, and the first pass's unit order with the sort behind it (indices | keys in | keys out |
-// radix-sort temp storage).  The context's for cf_toon / cf_chain, a run's own for cf_run_enqueue.
+// radix-sort temp storage).  The context's for cf_toon and cf_run_batch, a run's own for cf_run_enqueue.
 struct ToonWs {
   void* scratch;
   uint64_t scratch_bytes;
@@ -341,7 +341,7 @@ static int toon_enqueue(cf_ctx* ctx, cf_batch* b, uint32_t flags, uint8_t* d_out
   return CF_OK;
 }
 
-// the context's TOON workspace (cf_toon, cf_chain, cf_run_batch), grown on demand
+// the context's TOON workspace (cf_toon, cf_run_batch), grown on demand
 static int toon_ctx_ws(cf_ctx* ctx, const cf_batch* b, uint32_t flags, cudaStream_t st, ToonWs* ws) {
   const uint64_t need = toon_scratch_need(b->nbytes, b->n);
   if (need > ctx->toon_scratch_bytes) {
@@ -372,22 +372,6 @@ static int toon_launch(cf_ctx* ctx, cf_batch* b, uint32_t flags, uint8_t* d_out,
 int cf_toon(cf_ctx* ctx, cf_batch* b, uint32_t flags, uint8_t* d_out, uint32_t* d_out_len, int32_t* d_status, void* cuda_stream) {
   if (!ctx || !b || !b->n || !d_out || !d_out_len || !d_status) return CF_E_BADARG;
   return toon_launch(ctx, b, flags, d_out, d_out_len, d_status, nullptr, (cudaStream_t)cuda_stream);
-}
-
-int cf_chain(cf_ctx* ctx, cf_prog* prog, cf_batch* b, uint32_t stage_mask, uint32_t toon_flags, uint64_t* d_bitmaps, const uint8_t* d_unit_stages,
-             uint8_t* d_out, uint32_t* d_out_len, int32_t* d_status, void* cuda_stream) {
-  if (!ctx || !b || !b->n) return CF_E_BADARG;
-  if (stage_mask & ~(CF_STAGE_SCAN | CF_STAGE_TOON)) { ctx->err = "cf_chain runs CF_STAGE_SCAN / CF_STAGE_TOON; the other stages need cf_run_batch"; return CF_E_BADARG; }
-  int rc;
-  if (stage_mask & CF_STAGE_SCAN) {
-    if (!prog || !d_bitmaps) return CF_E_BADARG;
-    if ((rc = cf_scan(ctx, prog, b, d_bitmaps, cuda_stream))) return rc;
-  }
-  if (stage_mask & CF_STAGE_TOON) {
-    if (!d_out || !d_out_len || !d_status) return CF_E_BADARG;
-    if ((rc = toon_launch(ctx, b, toon_flags, d_out, d_out_len, d_status, d_unit_stages, (cudaStream_t)cuda_stream))) return rc;
-  }
-  return CF_OK;
 }
 
 #ifdef CF_TOON_PHASES
@@ -851,62 +835,9 @@ int cf_run_finish(cf_ctx* ctx, cf_run* run, uint64_t* needed) {
   return rc;
 }
 
-// CF_STAGE_MASK: the scan (and the substitution's verdict flags) and request_logging_masking on one upload; the masking kernel
-// gathers its own texts.
-static int run_batch_mask(cf_ctx* ctx, cf_prog* prog, cf_batch* b, const uint8_t* stream, uint64_t stream_bytes, const uint64_t* offsets, uint32_t n_units,
-                          uint32_t stage_mask, const uint8_t* unit_stages, int mask_max_depth, cf_verdict* verdicts, uint64_t* bitmaps_full,
-                          uint8_t* out_bytes, uint64_t out_cap, uint64_t* out_offsets, uint64_t* out_needed) {
-  const uint32_t W = prog ? prog->W : 1;
-  // pinned staging: bitmaps | substitution descriptors
-  const size_t o_sub = (((stage_mask & CF_STAGE_SCAN) ? (size_t)n_units * W * 8 : 0) + 15) & ~(size_t)15;
-  int rc = cf_stage_reserve(ctx, o_sub + ((stage_mask & CF_STAGE_SUB) ? cf_sub_stage_bytes(n_units) : 0));
-  if (rc) return rc;
-  uint8_t* hs = (uint8_t*)ctx->h_stage;
-  if (stream && (rc = cf_batch_upload(ctx, b, stream, stream_bytes, offsets, n_units, nullptr))) return rc;
-  for (uint32_t i = 0; i < n_units; ++i) { verdicts[i].match_bitmap = 0; verdicts[i].flags = 0; verdicts[i].out_len = 0; verdicts[i].aux = 0; verdicts[i].reserved = 0; }
-  if (stage_mask & CF_STAGE_SCAN) {
-    const uint64_t* bm = (const uint64_t*)hs;
-    if ((rc = cf_dev_reserve(ctx, ctx->tmp[6], (size_t)n_units * W * 8))) return rc;
-    if ((rc = cf_scan(ctx, prog, b, (uint64_t*)ctx->tmp[6].p, nullptr))) return rc;
-    CF_CUDA(ctx, cudaMemcpy(hs, ctx->tmp[6].p, (size_t)n_units * W * 8, cudaMemcpyDeviceToHost));
-    if (bitmaps_full) memcpy(bitmaps_full, bm, (size_t)n_units * W * 8);
-    std::vector<uint64_t> rule_mask(W, 0);
-    for (int pi : prog->ordered_pat) rule_mask[(size_t)pi / 64] |= 1ull << (pi % 64);
-    std::vector<uint32_t> dirty;
-    for (uint32_t i = 0; i < n_units; ++i) {
-      verdicts[i].match_bitmap = bm[(size_t)i * W];
-      if ((stage_mask & CF_STAGE_SUB) && (!unit_stages || (unit_stages[i] & CF_STAGE_SUB))) {
-        bool d = false;
-        for (uint32_t w = 0; w < W; ++w) if (bm[(size_t)i * W + w] & rule_mask[w]) { d = true; break; }
-        if (d) dirty.push_back(i);
-      }
-    }
-    const uint64_t* rec = nullptr;
-    if (!dirty.empty()) {
-      if ((rc = cf_sub_device(ctx, prog, b, offsets, dirty.data(), (uint32_t)dirty.size(), 0, hs + o_sub, &rec))) return rc;
-      for (size_t k = 0; k < dirty.size(); ++k) {
-        verdicts[dirty[k]].flags |= CF_V_REWRITTEN;
-        verdicts[dirty[k]].out_len = (uint32_t)rec[2 * k + 1];
-      }
-    }
-  }
-  std::vector<int32_t> mst(n_units);
-  std::vector<uint64_t> moff((size_t)n_units + 1);
-  uint64_t need = 0;
-  rc = cf_mask_resident(ctx, b, mask_max_depth, out_bytes, out_cap, moff.data(), mst.data(), &need);
-  if (out_needed) *out_needed = need;
-  if (rc) return rc;
-  for (uint32_t i = 0; i < n_units; ++i) {
-    out_offsets[i] = moff[i];
-    verdicts[i].aux = mst[i];
-    if (mst[i] == CF_MASK_OK) { verdicts[i].flags |= CF_V_MASKED; verdicts[i].out_len = (uint32_t)(moff[i + 1] - moff[i]); }
-  }
-  out_offsets[n_units] = moff[n_units];
-  return CF_OK;
-}
-
 // ---- the fused chain with host buffers (include/cfgpu.h): one H2D of the stream, cf_run_enqueue + cf_run_finish on the context's
 // run (legacy stream), then verdicts, offsets and only the produced texts cross PCIe back through the context's pinned staging.
+// With CF_STAGE_MASK the run (SCAN / SUB, when asked for) gives the verdicts, and the masking kernel then the texts, statuses and offsets.
 int cf_run_batch(cf_ctx* ctx, cf_prog* prog, cf_batch* b, const uint8_t* stream, uint64_t stream_bytes, const uint64_t* offsets, uint32_t n_units,
                  uint32_t stage_mask, const uint8_t* unit_stages, uint32_t toon_flags, int mask_max_depth, cf_verdict* verdicts, uint64_t* bitmaps_full,
                  uint8_t* out_bytes, uint64_t out_cap, uint64_t* out_offsets, uint64_t* out_needed) {
@@ -918,9 +849,9 @@ int cf_run_batch(cf_ctx* ctx, cf_prog* prog, cf_batch* b, const uint8_t* stream,
   struct Nvtx { Nvtx(const char* n) { nvtxRangePushA(n); } ~Nvtx() { nvtxRangePop(); } } nvtx_call("cf_run_batch");   // ranges: assemble (caller) | h2d | kernels | d2h
   // every return, error returns included, waits for the run's streams: nothing the next call's buffers are reused for stays in flight
   struct Drain { cf_ctx* c; ~Drain() { if (c->run) cudaStreamSynchronize(c->run->side); cudaStreamSynchronize(0); } } drain{ctx};
-  if (stage_mask & CF_STAGE_MASK)
-    return run_batch_mask(ctx, prog, b, stream, stream_bytes, offsets, n_units, stage_mask, unit_stages, mask_max_depth, verdicts, bitmaps_full, out_bytes,
-                          out_cap, out_offsets, out_needed);
+  const bool mask = (stage_mask & CF_STAGE_MASK) != 0;
+  stage_mask &= ~CF_STAGE_MASK;
+  const bool keep = !mask && (toon_flags & CF_RUN_OUTPUTS_RESIDENT) != 0;
   const uint32_t W = prog ? prog->W : 1;
   int rc;
   if (stream) {
@@ -929,76 +860,89 @@ int cf_run_batch(cf_ctx* ctx, cf_prog* prog, cf_batch* b, const uint8_t* stream,
     nvtxRangePop();
     if (rc) return rc;
   }
-  if (!ctx->run || ctx->run->max_units < n_units || ctx->run->max_bytes < stream_bytes) {     // the context's run, grown with the batches
-    const uint64_t arena = ctx->run ? ctx->run->arena_bytes : (1ull << 20);
-    cf_run_free(ctx->run);
-    ctx->run = nullptr;
-    if ((rc = run_create(ctx, n_units + n_units / 4, stream_bytes + stream_bytes / 4 + 4096, arena, false, &ctx->run))) return rc;
-  }
-  cf_run* run = ctx->run;
-  if (stage_mask & CF_STAGE_TOON) {       // the context's TOON workspace, lent to its run: TOON output in tmp[0], lengths | statuses in tmp[2]
-    ToonWs ws;
-    if ((rc = toon_ctx_ws(ctx, b, 0, 0, &ws)) || (rc = cf_dev_reserve(ctx, ctx->tmp[0], stream_bytes + 16)) ||
-        (rc = cf_dev_reserve(ctx, ctx->tmp[2], (size_t)n_units * 8)))
-      return rc;
-    run->d_toon_scratch = ws.scratch; run->toon_scratch_bytes = ws.scratch_bytes;
-    run->d_toon_order = ws.order; run->d_toon_sort = ws.sort; run->toon_sort_bytes = ws.sort_bytes;
-    run->d_toon_out = (uint8_t*)ctx->tmp[0].p;
-    run->d_toon_ls = (uint32_t*)ctx->tmp[2].p;
-  }
-  // pinned staging: unit_stages on the way in; verdicts | out_offsets | bitmaps on the way out
-  const bool keep = (toon_flags & CF_RUN_OUTPUTS_RESIDENT) != 0;
-  const size_t o_oo = ((size_t)n_units * sizeof(cf_verdict) + 15) & ~(size_t)15, o_bm = (o_oo + ((size_t)n_units + 1) * 8 + 15) & ~(size_t)15;
-  const size_t bm_bytes = (stage_mask & CF_STAGE_SCAN) ? (size_t)n_units * W * 8 : 0;
-  if ((rc = cf_stage_reserve(ctx, std::max(o_bm + bm_bytes, (size_t)n_units)))) return rc;
-  uint8_t* hs = (uint8_t*)ctx->h_stage;
-  if ((rc = cf_dev_reserve(ctx, ctx->tmp[1], (size_t)n_units * sizeof(cf_verdict))) || (rc = cf_dev_reserve(ctx, ctx->tmp[3], ((size_t)n_units + 1) * 8)) ||
-      (bm_bytes && (rc = cf_dev_reserve(ctx, ctx->tmp[6], bm_bytes))) ||
-      (rc = cf_dev_reserve(ctx, ctx->tmp[4], std::max<uint64_t>(16, keep ? stream_bytes : std::min(out_cap, stream_bytes)))))
-    return rc;
-  uint8_t* d_us = nullptr;
-  if (unit_stages) {
-    if ((rc = cf_dev_reserve(ctx, ctx->tmp[7], n_units))) return rc;
-    d_us = (uint8_t*)ctx->tmp[7].p;
-    memcpy(hs, unit_stages, n_units);
-    CF_CUDA(ctx, cudaMemcpyAsync(d_us, hs, n_units, cudaMemcpyHostToDevice, 0));
-  }
-  cf_verdict* d_v = (cf_verdict*)ctx->tmp[1].p;
-  uint64_t* d_oo = (uint64_t*)ctx->tmp[3].p;
-  // the device buffer takes what the caller can take (all of it when the texts stay resident); a shortfall of the device buffer alone
-  // is made up below by growing it and gathering again
-  const uint64_t dcap = keep ? ctx->tmp[4].cap : (out_bytes ? std::min<uint64_t>(ctx->tmp[4].cap, out_cap) : 0);
-  nvtxRangePushA("cf_run_batch:kernels");
-  rc = cf_run_enqueue(ctx, prog, b, run, stage_mask, d_us, toon_flags, d_v, bm_bytes ? (uint64_t*)ctx->tmp[6].p : nullptr, d_oo, (uint8_t*)ctx->tmp[4].p,
-                      dcap, nullptr);
-  uint64_t total = 0;
-  bool out_short = false;
-  if (!rc) rc = run_finish(ctx, run, offsets, &total, &out_short);
-  nvtxRangePop();
-  if (out_short && (keep || (out_bytes && total <= out_cap))) {
-    if ((rc = cf_dev_reserve(ctx, ctx->tmp[4], total))) return rc;
-    run->d_out = (uint8_t*)ctx->tmp[4].p;
-    run->out_cap = total;
-    if ((rc = run_gather(ctx, run))) return rc;
-    CF_CUDA(ctx, cudaStreamSynchronize(0));
-  }
-  const int grown = run_grow_arena(ctx, run);
-  if (rc && !out_short) return rc;
-  if (grown) return grown;
-  Nvtx nvtx_d2h("cf_run_batch:d2h");
-  if ((rc = cf_stage_reserve(ctx, o_bm + bm_bytes))) return rc;    // a deferred unit's substitution may have grown the staging
-  hs = (uint8_t*)ctx->h_stage;
-  CF_CUDA(ctx, cudaMemcpyAsync(hs, d_v, (size_t)n_units * sizeof(cf_verdict), cudaMemcpyDeviceToHost, 0));
-  CF_CUDA(ctx, cudaMemcpyAsync(hs + o_oo, d_oo, ((size_t)n_units + 1) * 8, cudaMemcpyDeviceToHost, 0));
-  if (bitmaps_full && bm_bytes) CF_CUDA(ctx, cudaMemcpyAsync(hs + o_bm, ctx->tmp[6].p, bm_bytes, cudaMemcpyDeviceToHost, 0));
-  const bool fits = keep || (total <= out_cap && (out_bytes || !total));
-  if (fits && !keep && total) CF_CUDA(ctx, cudaMemcpyAsync(out_bytes, ctx->tmp[4].p, total, cudaMemcpyDeviceToHost, 0));
-  CF_CUDA(ctx, cudaStreamSynchronize(0));
-  memcpy(verdicts, hs, (size_t)n_units * sizeof(cf_verdict));
-  memcpy(out_offsets, hs + o_oo, ((size_t)n_units + 1) * 8);
-  if (bitmaps_full && bm_bytes) memcpy(bitmaps_full, hs + o_bm, bm_bytes);
-  if (out_needed) *out_needed = total;
   ctx->run_out = nullptr; ctx->run_out_bytes = 0;
+  uint64_t total = 0;
+  bool fits = true;
+  if (mask && !stage_mask) memset(verdicts, 0, (size_t)n_units * sizeof(cf_verdict));    // masking alone: no run
+  else {
+    if (!ctx->run || ctx->run->max_units < n_units || ctx->run->max_bytes < stream_bytes) {     // the context's run, grown with the batches
+      const uint64_t arena = ctx->run ? ctx->run->arena_bytes : (1ull << 20);
+      cf_run_free(ctx->run);
+      ctx->run = nullptr;
+      if ((rc = run_create(ctx, n_units + n_units / 4, stream_bytes + stream_bytes / 4 + 4096, arena, false, &ctx->run))) return rc;
+    }
+    cf_run* run = ctx->run;
+    if (stage_mask & CF_STAGE_TOON) {       // the context's TOON workspace, lent to its run: TOON output in tmp[0], lengths | statuses in tmp[2]
+      ToonWs ws;
+      if ((rc = toon_ctx_ws(ctx, b, 0, 0, &ws)) || (rc = cf_dev_reserve(ctx, ctx->tmp[0], stream_bytes + 16)) ||
+          (rc = cf_dev_reserve(ctx, ctx->tmp[2], (size_t)n_units * 8)))
+        return rc;
+      run->d_toon_scratch = ws.scratch; run->toon_scratch_bytes = ws.scratch_bytes;
+      run->d_toon_order = ws.order; run->d_toon_sort = ws.sort; run->toon_sort_bytes = ws.sort_bytes;
+      run->d_toon_out = (uint8_t*)ctx->tmp[0].p;
+      run->d_toon_ls = (uint32_t*)ctx->tmp[2].p;
+    }
+    // pinned staging: unit_stages on the way in; verdicts | out_offsets | bitmaps on the way out
+    const size_t o_oo = ((size_t)n_units * sizeof(cf_verdict) + 15) & ~(size_t)15, o_bm = (o_oo + ((size_t)n_units + 1) * 8 + 15) & ~(size_t)15;
+    const size_t bm_bytes = (stage_mask & CF_STAGE_SCAN) ? (size_t)n_units * W * 8 : 0;
+    if ((rc = cf_stage_reserve(ctx, std::max(o_bm + bm_bytes, (size_t)n_units)))) return rc;
+    uint8_t* hs = (uint8_t*)ctx->h_stage;
+    if ((rc = cf_dev_reserve(ctx, ctx->tmp[1], (size_t)n_units * sizeof(cf_verdict))) || (rc = cf_dev_reserve(ctx, ctx->tmp[3], ((size_t)n_units + 1) * 8)) ||
+        (bm_bytes && (rc = cf_dev_reserve(ctx, ctx->tmp[6], bm_bytes))) ||
+        (rc = cf_dev_reserve(ctx, ctx->tmp[4], std::max<uint64_t>(16, keep ? stream_bytes : std::min(out_cap, stream_bytes)))))
+      return rc;
+    uint8_t* d_us = nullptr;
+    if (unit_stages) {
+      if ((rc = cf_dev_reserve(ctx, ctx->tmp[7], n_units))) return rc;
+      d_us = (uint8_t*)ctx->tmp[7].p;
+      memcpy(hs, unit_stages, n_units);
+      CF_CUDA(ctx, cudaMemcpyAsync(d_us, hs, n_units, cudaMemcpyHostToDevice, 0));
+    }
+    cf_verdict* d_v = (cf_verdict*)ctx->tmp[1].p;
+    uint64_t* d_oo = (uint64_t*)ctx->tmp[3].p;
+    // the device buffer takes what the caller can take (all of it when the texts stay resident); a shortfall of the device buffer alone
+    // is made up below by growing it and gathering again.  Masking returns no rewritten texts: the run gathers none, and the
+    // CF_E_CAPACITY its finish then reports for rewritten units is expected.
+    uint8_t* d_out = mask ? nullptr : (uint8_t*)ctx->tmp[4].p;
+    const uint64_t dcap = keep ? ctx->tmp[4].cap : (d_out && out_bytes ? std::min<uint64_t>(ctx->tmp[4].cap, out_cap) : 0);
+    nvtxRangePushA("cf_run_batch:kernels");
+    rc = cf_run_enqueue(ctx, prog, b, run, stage_mask, d_us, toon_flags, d_v, bm_bytes ? (uint64_t*)ctx->tmp[6].p : nullptr, d_oo, d_out, dcap, nullptr);
+    bool out_short = false;
+    if (!rc) rc = run_finish(ctx, run, offsets, &total, &out_short);
+    nvtxRangePop();
+    if (out_short && d_out && (keep || (out_bytes && total <= out_cap))) {
+      if ((rc = cf_dev_reserve(ctx, ctx->tmp[4], total))) return rc;
+      run->d_out = (uint8_t*)ctx->tmp[4].p;
+      run->out_cap = total;
+      if ((rc = run_gather(ctx, run))) return rc;
+      CF_CUDA(ctx, cudaStreamSynchronize(0));
+    }
+    const int grown = run_grow_arena(ctx, run);
+    if (rc && !out_short) return rc;
+    if (grown) return grown;
+    Nvtx nvtx_d2h("cf_run_batch:d2h");
+    if ((rc = cf_stage_reserve(ctx, o_bm + bm_bytes))) return rc;    // a deferred unit's substitution may have grown the staging
+    hs = (uint8_t*)ctx->h_stage;
+    CF_CUDA(ctx, cudaMemcpyAsync(hs, d_v, (size_t)n_units * sizeof(cf_verdict), cudaMemcpyDeviceToHost, 0));
+    CF_CUDA(ctx, cudaMemcpyAsync(hs + o_oo, d_oo, ((size_t)n_units + 1) * 8, cudaMemcpyDeviceToHost, 0));
+    if (bitmaps_full && bm_bytes) CF_CUDA(ctx, cudaMemcpyAsync(hs + o_bm, ctx->tmp[6].p, bm_bytes, cudaMemcpyDeviceToHost, 0));
+    fits = keep || (total <= out_cap && (out_bytes || !total));
+    if (fits && d_out && !keep && total) CF_CUDA(ctx, cudaMemcpyAsync(out_bytes, ctx->tmp[4].p, total, cudaMemcpyDeviceToHost, 0));
+    CF_CUDA(ctx, cudaStreamSynchronize(0));
+    memcpy(verdicts, hs, (size_t)n_units * sizeof(cf_verdict));
+    memcpy(out_offsets, hs + o_oo, ((size_t)n_units + 1) * 8);
+    if (bitmaps_full && bm_bytes) memcpy(bitmaps_full, hs + o_bm, bm_bytes);
+  }
+  if (mask) {     // the masked bodies are the output: the mask's texts, offsets, size and CF_E_CAPACITY; its statuses patch the records
+    std::vector<int32_t> mst(n_units);
+    if ((rc = cf_mask_resident(ctx, b, mask_max_depth, out_bytes, out_cap, out_offsets, mst.data(), out_needed))) return rc;
+    for (uint32_t i = 0; i < n_units; ++i) {
+      verdicts[i].aux = mst[i];
+      if (mst[i] == CF_MASK_OK) { verdicts[i].flags |= CF_V_MASKED; verdicts[i].out_len = (uint32_t)(out_offsets[i + 1] - out_offsets[i]); }
+    }
+    return CF_OK;
+  }
+  if (out_needed) *out_needed = total;
   if (!fits) { ctx->err = "output buffer too small"; return CF_E_CAPACITY; }
   if (keep) {
     ctx->run_out = total ? (const uint8_t*)ctx->tmp[4].p : nullptr;

@@ -1,4 +1,4 @@
-"""The device-resident entry points (cf_scan, cf_toon, cf_chain, cf_json_index, cf_run_batch with the batch or the outputs
+"""The device-resident entry points (cf_scan, cf_toon, cf_run_enqueue, cf_json_index, cf_run_batch with the batch or the outputs
 left in HBM), one long-lived Batch that takes uploads of very different sizes one after the other (what the product's
 batchers do), and the host-side cache of a batch's unit lengths in cf_sub_host across a freed and re-allocated batch.
 Everything is checked against the oracles and against the host-buffer entry points on a fresh batch."""
@@ -93,7 +93,7 @@ def _toon_texts(out, out_len, status, offs):
     return st, [o[int(offs[i]):int(offs[i]) + int(ln[i])].tobytes().decode() if st[i] == engine.TOON_CONVERTED else None for i in range(len(st))]
 
 
-def test_cf_toon_and_cf_chain_device_resident():
+def test_cf_toon_and_run_enqueue_device_resident():
     import torch
 
     ctx = engine.Context.get()
@@ -110,22 +110,23 @@ def test_cf_toon_and_cf_chain_device_resident():
     st, texts = _toon_texts(out, out_len, status, offs)
     assert texts == [toon_oracle(u) for u in units]
     assert (st == engine.TOON_CONVERTED).sum() >= 8
-    # cf_chain: scan + TOON on the resident batch; units whose stage mask leaves out TOON come back SKIPPED
+    # cf_run_enqueue: scan + TOON on the resident batch; units whose stage mask leaves out TOON come back SKIPPED
     stages = np.array([N.CF_STAGE_SCAN | (N.CF_STAGE_TOON if i % 3 else 0) for i in range(n)], dtype=np.uint8)
     d_stages = torch.from_numpy(stages).cuda()
     bm = torch.full((n * prog.words,), -1, dtype=torch.int64, device="cuda")
-    out, out_len, status = _toon_buffers(len(stream), n)
-    with ctx.lock:
-        ctx.check(ctx.lib.cf_chain(ctx.h, prog.h, batch.h, N.CF_STAGE_SCAN | N.CF_STAGE_TOON, 1, ptr(bm), ptr(d_stages), ptr(out), ptr(out_len), ptr(status), None),
-                  "cf_chain")
-    torch.cuda.synchronize()
-    st, texts = _toon_texts(out, out_len, status, offs)
+    v = torch.zeros(n * 24, dtype=torch.uint8, device="cuda")
+    oo = torch.zeros(n + 1, dtype=torch.int64, device="cuda")
+    out = torch.zeros(len(stream), dtype=torch.uint8, device="cuda")
+    run = engine.Run(ctx, n, len(stream))
+    run.enqueue(prog, batch, N.CF_STAGE_SCAN | N.CF_STAGE_TOON, d_stages, 1, v, oo, out, bm)
+    assert run.finish() == 0
+    v, oo, out = v.cpu().numpy().view(engine.VERDICT_DTYPE), oo.cpu().numpy(), out.cpu().numpy()
     assert engine.bitmaps_to_ints(bm.cpu().numpy().view(np.uint64), n, prog.words) == oracle_bits(units, MORE)
     for i, u in enumerate(units):
         if stages[i] & N.CF_STAGE_TOON:
-            assert texts[i] == toon_oracle(u), i
+            assert (out[oo[i]:oo[i + 1]].tobytes().decode() if v["flags"][i] & N.CF_V_TOON else None) == toon_oracle(u), i
         else:
-            assert st[i] == engine.TOON_SKIPPED, i
+            assert v["aux"][i] == engine.TOON_SKIPPED, i
 
 
 def test_cf_json_index_device_resident_matches_host_entry_point():
