@@ -144,8 +144,10 @@ int cf_sub_host(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint32_t* units, uin
 /* mask_sensitive_json_bytes(payload, max_depth) per unit (one JSON request body per unit):
  * crates/request_logging_masking_native_extension/src/lib.rs:346-360.  Masked compact JSON of every
  * unit with status CF_MASK_OK is returned back to back in out_bytes / out_offsets[n+1].
- * status: CF_MASK_OK, CF_MASK_PARSE_ERROR (the crate raises ValueError), CF_MASK_UNSUPPORTED (beyond
- * device limits: nesting > 64, number > 3200 bits — the caller must fail loudly). */
+ * status: CF_MASK_OK, CF_MASK_PARSE_ERROR (the crate raises ValueError: invalid JSON, a number out of
+ * binary64's range anywhere in the document, nesting deeper than serde_json's 127 levels),
+ * CF_MASK_UNSUPPORTED (beyond the device limits: a number literal longer than the 3200-bit workspace, or a
+ * body over 768 MiB — the caller must fail loudly).  Outputs of any size are returned. */
 #define CF_MASK_OK 0
 #define CF_MASK_PARSE_ERROR 2
 #define CF_MASK_UNSUPPORTED 6

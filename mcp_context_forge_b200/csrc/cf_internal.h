@@ -207,5 +207,5 @@ static const uint32_t TOON_ONLY_FALLBACK = 0x100u;     // internal flag of toon_
 void cf_launch_toon_seq(uint32_t blocks, cudaStream_t st, const uint8_t* stream, const uint64_t* offsets, uint32_t n_units, cfj::JNode* nodes, uint8_t* out,
                         uint32_t* out_len, int32_t* status, uint32_t flags, uint32_t upw);
 void cf_launch_mask_seq(uint32_t blocks, const uint8_t* stream, const uint64_t* offsets, uint32_t n_units, cfj::JNode* nodes, uint32_t* idx, uint8_t* out,
-                        uint32_t* out_len, int32_t* status, int max_depth, uint32_t upw);
+                        uint32_t* out_len, int32_t* status, int max_depth, uint32_t upw, const uint32_t* retry, const uint64_t* out_off);
 void cf_launch_classify_keys(uint32_t blocks, const uint8_t* stream, const uint64_t* offsets, uint32_t n_units, uint8_t* sensitive);

@@ -472,13 +472,20 @@ static int cf_mask_resident(cf_ctx* ctx, cf_batch* b, int max_depth, uint8_t* ou
   std::vector<uint32_t> lens(n_units);
   const uint32_t upw = units_per_warp(ctx, n_units);
   cf_launch_mask_seq(json_blocks(n_units, upw), b->d_buf + cf::FRONT_PAD, b->d_offsets, n_units, (cfj::JNode*)ctx->d_toon_scratch, d_idx, d_arena, d_len,
-                                                 d_st, max_depth, upw);
+                                                 d_st, max_depth, upw, nullptr, nullptr);
   ctx->launches++;
   CF_CUDA(ctx, cudaGetLastError());
   CF_CUDA(ctx, cudaMemcpy(lens.data(), d_len, (size_t)n_units * 4, cudaMemcpyDeviceToHost));
   CF_CUDA(ctx, cudaMemcpy(status, d_st, (size_t)n_units * 4, cudaMemcpyDeviceToHost));
+  // A unit whose output outgrew its 5 * len + 32 bytes (MS_OVERFLOW, lens = the length it needs) is masked again below, straight
+  // into its place in the gathered output.  Its offsets count that length already.
+  std::vector<uint32_t> retry;
   uint64_t total = 0;
-  for (uint32_t i = 0; i < n_units; ++i) { out_offsets[i] = total; total += lens[i]; }
+  for (uint32_t i = 0; i < n_units; ++i) {
+    if (status[i] == cfm::MS_OVERFLOW) retry.push_back(i);
+    out_offsets[i] = total;
+    total += lens[i];
+  }
   out_offsets[n_units] = total;
   if (out_needed) *out_needed = total;
   if (total > out_cap || (!out_bytes && total)) { ctx->err = "output buffer too small"; return CF_E_CAPACITY; }
@@ -486,9 +493,26 @@ static int cf_mask_resident(cf_ctx* ctx, cf_batch* b, int max_depth, uint8_t* ou
     if ((rc = cf_dev_reserve(ctx, ctx->tmp[4], total))) return rc;
     if ((rc = cf_stage_reserve(ctx, total))) return rc;
     CF_CUDA(ctx, cudaMemcpy(d_ooff, out_offsets, ((size_t)n_units + 1) * 8, cudaMemcpyHostToDevice));
+    if (!retry.empty()) {        // the gather copies nothing for them (their text is not in the arena)
+      for (uint32_t u : retry) lens[u] = 0;
+      CF_CUDA(ctx, cudaMemcpy(d_len, lens.data(), (size_t)n_units * 4, cudaMemcpyHostToDevice));
+    }
     compact_kernel<<<n_units, 128>>>(d_arena, 5, 32, b->d_offsets, d_len, d_ooff, (uint8_t*)ctx->tmp[4].p, n_units);
     ctx->launches++;
     CF_CUDA(ctx, cudaGetLastError());
+    if (!retry.empty()) {        // the unit list goes to the arena, which the gather has finished reading
+      const uint32_t nr = (uint32_t)retry.size();
+      uint32_t* d_retry = (uint32_t*)d_arena;
+      CF_CUDA(ctx, cudaMemcpy(d_retry, retry.data(), (size_t)nr * 4, cudaMemcpyHostToDevice));
+      const uint32_t rupw = units_per_warp(ctx, nr);
+      cf_launch_mask_seq(json_blocks(nr, rupw), b->d_buf + cf::FRONT_PAD, b->d_offsets, nr, (cfj::JNode*)ctx->d_toon_scratch, d_idx,
+                         (uint8_t*)ctx->tmp[4].p, d_len, d_st, max_depth, rupw, d_retry, d_ooff);
+      ctx->launches++;
+      CF_CUDA(ctx, cudaGetLastError());
+      CF_CUDA(ctx, cudaMemcpy(status, d_st, (size_t)n_units * 4, cudaMemcpyDeviceToHost));
+      for (uint32_t u : retry)
+        if (status[u] != cfm::MS_OK) { ctx->err = "mask_kernel: a unit retried with the room it asked for did not fit"; return CF_E_CUDA; }
+    }
     CF_CUDA(ctx, cudaMemcpy(ctx->h_stage, ctx->tmp[4].p, total, cudaMemcpyDeviceToHost));
     memcpy(out_bytes, ctx->h_stage, total);
   }

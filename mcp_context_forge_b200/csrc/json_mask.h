@@ -15,10 +15,34 @@ namespace cfm {
 using cfj::Big;
 using cfj::Dbl;
 using cfj::JNode;
-using cfj::Out;
 using cfj::StrIter;
 
 enum : int { MS_OK = 0, MS_PARSE_ERROR = 2, MS_UNSUPPORTED = 6, MS_OVERFLOW = 7 };
+
+// serde_json's recursion limit: remaining_depth starts at 128 and the parse fails when an opening bracket brings it to 0, so a
+// document holds at most 127 nested containers.  The mask path parses exactly that deep; one level more is a parse error.
+static const int MASK_MAXD = 127;
+
+// Output cursor of the masking walk.  Past its cap it stops writing but keeps counting, so that a unit whose output outgrows its
+// room reports the exact length it needs (saturating at 0xFFFFFFFF).
+struct Out {
+  uint8_t* p;
+  uint32_t n, cap;
+  bool over;
+  CF_HD void put(uint32_t c) { if (n < cap) p[n++] = (uint8_t)c; else { over = true; if (n != 0xFFFFFFFFu) ++n; } }
+  CF_HD void puts(const char* z) { while (*z) put((uint8_t)*z++); }
+  CF_HD void put_cp(uint32_t cp) {
+    if (cp < 0x80) put(cp);
+    else if (cp < 0x800) { put(0xC0 | (cp >> 6)); put(0x80 | (cp & 63)); }
+    else if (cp < 0x10000) { put(0xE0 | (cp >> 12)); put(0x80 | ((cp >> 6) & 63)); put(0x80 | (cp & 63)); }
+    else { put(0xF0 | (cp >> 18)); put(0x80 | ((cp >> 12) & 63)); put(0x80 | ((cp >> 6) & 63)); put(0x80 | (cp & 63)); }
+  }
+  CF_HD void put_uint(uint32_t v) {
+    uint8_t b[10]; int k = 0;
+    do { b[k++] = (uint8_t)('0' + v % 10); v /= 10; } while (v);
+    while (k) put(b[--k]);
+  }
+};
 
 // ------------------------------------------------------------------------------------------------
 // sensitive-key classifier (streaming over the decoded key; no buffer for the normalised key)
@@ -179,37 +203,19 @@ CF_HD bool exact_digits(const Dbl& d, NumWork& w, uint32_t* nd_out, int* kk_out)
   return true;
 }
 
-// shortest digit string that parses back to exactly `d` (binary search on the precision; each probe is
-// an exact round-half-even of the decimal expansion followed by an exact decimal->binary64 conversion)
+// shortest digit string that parses back to exactly `d`: binary search on the precision p.  A probe takes the p-digit decimal
+// nearest to `d` (exact round-half-even of the decimal expansion) and, when that one does not parse back to `d`, the p-digit
+// decimal on the other side of `d`.  The second one matters at a power of two: there the interval that rounds to `d` is half
+// as wide below `d` as above it, so the nearest decimal can fall out of it while the farther one is inside.  "Some p-digit
+// decimal parses back" is monotone in p, which keeps the binary search valid, and the nearer of two that both parse back wins.
 CF_HD bool shortest_digits(const Dbl& d, NumWork& w, uint8_t* out_ds, int* out_n, int* out_kk) {
   uint32_t nd;
   int kk;
   if (!exact_digits(d, w, &nd, &kk)) return false;
   const uint8_t* D = w.digits;
   uint8_t* txt = w.digits + w.digits_cap - 24;     // "dddddddddddddddddE" scratch lives at the buffer's tail
-  int lo = 1, hi = nd < 17 ? (int)nd : 17;          // 17 significant digits always round-trip
-  int best_n = 0, best_kk = 0;
-  uint8_t best[17];
-  while (lo <= hi) {
-    const int p = (lo + hi) >> 1;
-    uint8_t c[18];
-    int ckk = kk;
-    for (int i = 0; i < p; ++i) c[i] = D[i];
-    if ((uint32_t)p < nd) {
-      bool up = false;
-      if (D[p] > '5') up = true;
-      else if (D[p] == '5') {
-        bool rest = false;
-        for (uint32_t i = (uint32_t)p + 1; i < nd; ++i) if (D[i] != '0') { rest = true; break; }
-        up = rest || ((D[p - 1] - '0') & 1);
-      }
-      if (up) {
-        int i = p - 1;
-        while (i >= 0 && c[i] == '9') { c[i] = '0'; --i; }
-        if (i >= 0) c[i]++; else { for (int j = p - 1; j > 0; --j) c[j] = c[j - 1]; c[0] = '1'; ++ckk; }
-      }
-    }
-    // text "c[0..p)e(ckk-p)"
+  // 0 / 1: whether "c[0..p)e(ckk-p)" parses back to d; -1: the workspace is too small
+  auto round_trips = [&](const uint8_t* c, int p, int ckk) -> int {
     uint32_t tl = 0;
     for (int i = 0; i < p; ++i) txt[tl++] = c[i];
     txt[tl++] = 'e';
@@ -219,9 +225,40 @@ CF_HD bool shortest_digits(const Dbl& d, NumWork& w, uint8_t* out_ds, int* out_n
     do { eb[en++] = (uint8_t)('0' + ex % 10); ex /= 10; } while (ex);
     while (en) txt[tl++] = eb[--en];
     Dbl back;
-    if (!cfj::dec_to_double(txt, tl, &back, w.big2)) return false;
-    const bool same = !back.inf && back.m == d.m && (back.e == d.e || back.m == 0);
-    if (same) { best_n = p; best_kk = ckk; for (int i = 0; i < p; ++i) best[i] = c[i]; hi = p - 1; }
+    if (!cfj::dec_to_double(txt, tl, &back, w.big2)) return -1;
+    return !back.inf && back.m == d.m && (back.e == d.e || back.m == 0);
+  };
+  int lo = 1, hi = nd < 17 ? (int)nd : 17;          // 17 significant digits always round-trip
+  int best_n = 0, best_kk = 0;
+  uint8_t best[17];
+  while (lo <= hi) {
+    const int p = (lo + hi) >> 1;
+    uint8_t dn[17], upc[17];                         // D truncated to p digits, and one unit in the p-th digit above it
+    int up_kk = kk;
+    for (int i = 0; i < p; ++i) dn[i] = upc[i] = D[i];
+    bool exact = true, up = false;
+    for (uint32_t i = (uint32_t)p; i < nd; ++i) if (D[i] != '0') { exact = false; break; }
+    if (!exact) {
+      int i = p - 1;
+      while (i >= 0 && upc[i] == '9') { upc[i] = '0'; --i; }
+      if (i >= 0) upc[i]++; else { for (int j = p - 1; j > 0; --j) upc[j] = upc[j - 1]; upc[0] = '1'; ++up_kk; }
+      if (D[p] > '5') up = true;
+      else if (D[p] == '5') {
+        bool rest = false;
+        for (uint32_t i2 = (uint32_t)p + 1; i2 < nd; ++i2) if (D[i2] != '0') { rest = true; break; }
+        up = rest || ((D[p - 1] - '0') & 1);
+      }
+    }
+    const uint8_t* c = up ? upc : dn;
+    int ckk = up ? up_kk : kk;
+    int r = round_trips(c, p, ckk);
+    if (r < 0) return false;
+    if (!r && !exact) {
+      c = up ? dn : upc;
+      ckk = up ? kk : up_kk;
+      if ((r = round_trips(c, p, ckk)) < 0) return false;
+    }
+    if (r) { best_n = p; best_kk = ckk; for (int i = 0; i < p; ++i) best[i] = c[i]; hi = p - 1; }
     else lo = p + 1;
   }
   if (!best_n) return false;
@@ -293,6 +330,37 @@ CF_HD int emit_number_serde(Out& o, const uint8_t* s, const JNode& nd, NumWork& 
   return MS_OK;
 }
 
+// serde_json parses the whole document before masking it, so a number out of binary64's range fails the call wherever it sits,
+// printed, masked, below the depth cap or overwritten by a duplicate key: the mask path's parser runs this on every number.  Every literal under 10^308 is in range; one of 10^309 or more is not; only those in [10^308, 10^309) need the
+// exact conversion.  MS_OK, MS_PARSE_ERROR ("number out of range") or MS_UNSUPPORTED (longer than the workspace).
+CF_HD int number_in_range(const uint8_t* t, uint32_t len, uint32_t fl, NumWork& w) {
+  if (!(fl & cfj::JF_EXP) && len <= 308) return MS_OK;   // at most 308 integer digits
+  long long kk = 0;                                      // value in [10^(kk-1), 10^kk)
+  bool dot = false, any = false;
+  uint32_t p = (fl & cfj::JF_NEG) ? 1 : 0;
+  for (; p < len; ++p) {
+    const uint8_t c = t[p];
+    if (c == '.') { dot = true; continue; }
+    if (c == 'e' || c == 'E') break;
+    if (!any) { if (c == '0') { if (dot) --kk; continue; } any = true; }
+    if (!dot) ++kk;
+  }
+  if (!any) return MS_OK;                                // +-0
+  if (p < len) {
+    ++p;
+    bool en = false;
+    if (p < len && (t[p] == '+' || t[p] == '-')) { en = t[p] == '-'; ++p; }
+    long long ex = 0;
+    for (; p < len; ++p) if (ex < 100000) ex = ex * 10 + (t[p] - '0');
+    kk += en ? -ex : ex;
+  }
+  if (kk <= 308) return MS_OK;
+  if (kk >= 310) return MS_PARSE_ERROR;
+  Dbl d;
+  if (!cfj::dec_to_double(t, len, &d, w.big)) return MS_UNSUPPORTED;
+  return d.inf ? MS_PARSE_ERROR : MS_OK;
+}
+
 CF_HD void emit_json_string(Out& o, const uint8_t* s, const JNode& nd) {
   StrIter it{s + nd.off, s + nd.off + nd.len};
   o.put('"');
@@ -355,7 +423,7 @@ struct MFrame { uint32_t node, cur, i, seg; int depth; };   // depth = max_depth
 
 // emit value `v` given the depth budget `depth` of the call mask_json_value_inner(v, depth)
 CF_HD int mask_emit(const uint8_t* s, const JNode* N, Out& o, int max_depth, uint32_t* idx, uint32_t idx_cap, NumWork& w) {
-  MFrame st[cfj::MAXD + 1];
+  MFrame st[MASK_MAXD + 1];
   int sp = 0;
   uint32_t idx_used = 0;
   // returns true when a frame was pushed
@@ -402,7 +470,7 @@ CF_HD int mask_emit(const uint8_t* s, const JNode* N, Out& o, int max_depth, uin
       o.put(':');
       if (key_sensitive(s, N[k])) { o.puts("\"******\""); continue; }
       const int depth = f.depth;
-      if (sp > cfj::MAXD) { err = MS_UNSUPPORTED; break; }
+      if (sp > MASK_MAXD) { err = MS_UNSUPPORTED; break; }
       value(k + 1, depth, &err);
     } else {
       if (f.cur == 0) { o.put(']'); --sp; continue; }
@@ -411,7 +479,7 @@ CF_HD int mask_emit(const uint8_t* s, const JNode* N, Out& o, int max_depth, uin
       ++f.i;
       f.cur = N[x].next;
       const int depth = f.depth;
-      if (sp > cfj::MAXD) { err = MS_UNSUPPORTED; break; }
+      if (sp > MASK_MAXD) { err = MS_UNSUPPORTED; break; }
       value(x, depth, &err);
     }
   }
@@ -421,15 +489,26 @@ CF_HD int mask_emit(const uint8_t* s, const JNode* N, Out& o, int max_depth, uin
 CF_HD int mask_finish(int pr, const uint8_t* s, const JNode* nodes, uint32_t* idx, uint32_t idx_cap, uint8_t* out, uint32_t out_cap,
                       uint32_t* out_len, int max_depth, NumWork& w);
 
+// serde_json's parse: nesting up to its recursion limit, and every number in binary64's range
+struct RangeCheck {
+  NumWork* w;
+  CF_HD int operator()(const uint8_t* t, uint32_t len, uint32_t fl) const {
+    const int r = number_in_range(t, len, fl, *w);
+    return r == MS_OK ? cfj::PARSE_OK : r == MS_PARSE_ERROR ? cfj::PARSE_ERROR : cfj::PARSE_UNSUPPORTED;
+  }
+};
+
 // Whole per-unit pipeline: mask_sensitive_json_bytes(payload, max_depth).
 CF_HD int mask_process(const uint8_t* s, uint32_t n, JNode* nodes, uint32_t node_cap, uint32_t* idx, uint32_t idx_cap, uint8_t* out,
                        uint32_t out_cap, uint32_t* out_len, int max_depth, NumWork& w) {
   uint32_t count = 0;
-  int pr = cfj::json_parse(s, n, nodes, node_cap, &count);
+  RangeCheck check{&w};
+  int pr = cfj::json_parse_t<MASK_MAXD, cfj::PARSE_ERROR>(s, n, nodes, node_cap, &count, check);
   return mask_finish(pr, s, nodes, idx, idx_cap, out, out_cap, out_len, max_depth, w);
 }
 
-// the part after the parse (pr = PARSE_* of whichever parser built `nodes`)
+// the part after the parse (pr = PARSE_* of whichever parser built `nodes`).  MS_OVERFLOW: the output did not fit in out_cap
+// bytes, and *out_len is the length it needs.
 CF_HD int mask_finish(int pr, const uint8_t* s, const JNode* nodes, uint32_t* idx, uint32_t idx_cap, uint8_t* out, uint32_t out_cap,
                       uint32_t* out_len, int max_depth, NumWork& w) {
   if (pr == cfj::PARSE_ERROR) return MS_PARSE_ERROR;
@@ -438,9 +517,9 @@ CF_HD int mask_finish(int pr, const uint8_t* s, const JNode* nodes, uint32_t* id
   o.p = out; o.n = 0; o.cap = out_cap; o.over = false;
   int err = mask_emit(s, nodes, o, max_depth, idx, idx_cap, w);
   if (err) return err;
-  if (o.over) return MS_OVERFLOW;
+  if (o.over && o.n == 0xFFFFFFFFu) return MS_UNSUPPORTED;
   *out_len = o.n;
-  return MS_OK;
+  return o.over ? MS_OVERFLOW : MS_OK;
 }
 
 }  // namespace cfm

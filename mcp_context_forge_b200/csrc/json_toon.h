@@ -336,13 +336,39 @@ CF_HD bool scan_number(const uint8_t* s, uint32_t n, uint32_t* ppos, uint32_t* p
 // lives in thread-local arrays: a read-after-write through the node array in HBM costs an L2 round
 // trip per token, local memory stays in L1.  Nodes are written once, when complete.
 static const uint32_t KH_CAP = 512;        // key hashes of all currently open objects (an object whose hashes did not fit -> slow dedupe)
-CF_HD int json_parse(const uint8_t* s, uint32_t n, JNode* nodes, uint32_t cap, uint32_t* out_count) {
+
+// One bit per open container depth.  The 64-deep stack keeps a single word, so the TOON parsers compile as they always did.
+template <int D> struct DepthBits {
+  uint64_t w[(D + 63) / 64];
+  CF_HD void clear() { for (int i = 0; i < (D + 63) / 64; ++i) w[i] = 0; }
+  CF_HD bool get(int d) const { return (w[d >> 6] >> (d & 63)) & 1; }
+  CF_HD void set(int d) { w[d >> 6] |= 1ull << (d & 63); }
+  CF_HD void reset(int d) { w[d >> 6] &= ~(1ull << (d & 63)); }
+};
+template <> struct DepthBits<64> {
+  uint64_t w;
+  CF_HD void clear() { w = 0; }
+  CF_HD bool get(int d) const { return (w >> d) & 1; }
+  CF_HD void set(int d) { w |= 1ull << d; }
+  CF_HD void reset(int d) { w &= ~(1ull << d); }
+};
+
+struct NoNumberCheck {
+  CF_HD int operator()(const uint8_t*, uint32_t, uint32_t) const { return PARSE_OK; }
+};
+
+// D: deepest nesting held (a container deeper than D gives TOO_DEEP).  check(text, len, JF_* flags) sees every number as it is
+// scanned, before a duplicate key can overwrite it; a non-zero PARSE_* it returns ends the parse with that status.
+template <int D, int TOO_DEEP, class NumberCheck>
+CF_HD int json_parse_t(const uint8_t* s, uint32_t n, JNode* nodes, uint32_t cap, uint32_t* out_count, NumberCheck& check) {
   uint32_t pos = 0, nn = 0;
-  uint32_t st_node[MAXD], st_last[MAXD], st_len[MAXD], st_kh[MAXD];
+  uint32_t st_node[D], st_last[D], st_len[D], st_kh[D];
   uint32_t kh[KH_CAP];
   uint32_t khn = 0;                 // used entries of kh
-  uint64_t khbad = 0;               // bit d: the object at depth d has keys whose hashes did not fit
-  uint64_t objbits = 0;             // bit d: the container at depth d is an object
+  DepthBits<D> khbad;               // bit d: the object at depth d has keys whose hashes did not fit
+  DepthBits<D> objbits;             // bit d: the container at depth d is an object
+  khbad.clear();
+  objbits.clear();
   int sp = 0;
   bool member = false;              // the value being parsed belongs to an object member
   uint32_t member_hash = 0;
@@ -362,7 +388,7 @@ CF_HD int json_parse(const uint8_t* s, uint32_t n, JNode* nodes, uint32_t cap, u
         if (st_last[sp - 1]) nodes[st_last[sp - 1]].next = idx; else nodes[st_node[sp - 1]].off = idx;
         st_last[sp - 1] = idx;
         st_len[sp - 1]++;
-        if (khn < KH_CAP) kh[khn++] = h; else khbad |= 1ull << (sp - 1);
+        if (khn < KH_CAP) kh[khn++] = h; else khbad.set(sp - 1);
         while (pos < n && j_ws(s[pos])) ++pos;
         if (pos >= n || s[pos] != ':') return PARSE_ERROR;
         ++pos;
@@ -380,10 +406,10 @@ CF_HD int json_parse(const uint8_t* s, uint32_t n, JNode* nodes, uint32_t cap, u
       }
       member = false;
       if (c == '{' || c == '[') {
-        if (sp >= MAXD) return PARSE_UNSUPPORTED;
+        if (sp >= D) return TOO_DEEP;
         nodes[nn++] = JNode{c == '{' ? (uint32_t)J_OBJ : (uint32_t)J_ARR, 0, 0, keep_next};
         st_node[sp] = idx; st_last[sp] = 0; st_len[sp] = 0; st_kh[sp] = khn;
-        if (c == '{') objbits |= 1ull << sp; else objbits &= ~(1ull << sp);
+        if (c == '{') objbits.set(sp); else objbits.reset(sp);
         ++sp;
         ++pos;
         while (pos < n && j_ws(s[pos])) ++pos;
@@ -398,6 +424,7 @@ CF_HD int json_parse(const uint8_t* s, uint32_t n, JNode* nodes, uint32_t cap, u
       } else if (c == '-' || (c >= '0' && c <= '9')) {
         uint32_t p0 = pos, fl = 0;
         if (!scan_number(s, n, &pos, &fl)) return PARSE_ERROR;
+        if (const int r = check(s + p0, pos - p0, fl)) return r;
         nodes[nn++] = JNode{J_NUM | fl, p0, pos - p0, keep_next};
       } else if (c == 't' && pos + 4 <= n && s[pos + 1] == 'r' && s[pos + 2] == 'u' && s[pos + 3] == 'e') {
         nodes[nn++] = JNode{J_TRUE, pos, 4, keep_next}; pos += 4;
@@ -417,7 +444,7 @@ CF_HD int json_parse(const uint8_t* s, uint32_t n, JNode* nodes, uint32_t cap, u
       return PARSE_OK;
     }
     if (pos >= n) return PARSE_ERROR;
-    const bool is_obj = (objbits >> (sp - 1)) & 1;
+    const bool is_obj = objbits.get(sp - 1);
     uint32_t c = s[pos];
     if (c == ',') {
       ++pos;
@@ -434,8 +461,8 @@ CF_HD int json_parse(const uint8_t* s, uint32_t n, JNode* nodes, uint32_t cap, u
       // duplicate keys: the last value wins, the first position stays (Python dict / orjson).
       // Cheap screen on the hashes held in local memory; the node walk only runs when two hashes collide.
       const uint32_t kb = st_kh[sp];
-      bool maybe_dup = (khbad >> sp) & 1;
-      khbad &= ~(1ull << sp);
+      bool maybe_dup = khbad.get(sp);
+      khbad.reset(sp);
       if (!maybe_dup)
         for (uint32_t i = kb + 1; i < khn && !maybe_dup; ++i)
           for (uint32_t j = kb; j < i; ++j) if (kh[j] == kh[i]) { maybe_dup = true; break; }
@@ -463,6 +490,10 @@ CF_HD int json_parse(const uint8_t* s, uint32_t n, JNode* nodes, uint32_t cap, u
     nodes[cidx].len = clen;
     mode = M_AFTER;
   }
+}
+CF_HD int json_parse(const uint8_t* s, uint32_t n, JNode* nodes, uint32_t cap, uint32_t* out_count) {
+  NoNumberCheck none;
+  return json_parse_t<MAXD, PARSE_UNSUPPORTED>(s, n, nodes, cap, out_count, none);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -11,9 +11,10 @@ plus the batch forms the serving path should use (`*_batch`), which put many req
 packed stream and one kernel launch.  The sensitive-key classifier, the masking walk and the
 serde_json-compatible re-serialisation run on the GPU (csrc/json_mask.h).  Cookie splitting for the
 `cookie` header is host logic (a handful of bytes per request), restating lib.rs:199-231.
-Errors: invalid JSON raises ValueError like the crate (the middleware then takes its own Python
-path, mcpgateway/middleware/request_logging_middleware.py:299-305); payloads beyond the device
-limits raise RuntimeError — never a silent different answer.
+Errors: whatever serde_json rejects (invalid JSON, lone surrogates, numbers out of binary64's range,
+nesting deeper than 127 levels) raises ValueError like the crate (the middleware then takes its own
+Python path, mcpgateway/middleware/request_logging_middleware.py:299-305); number literals longer than
+the device's 3200-bit workspace raise RuntimeError — never a silent different answer.
 """
 from __future__ import annotations
 
@@ -43,7 +44,8 @@ def _batch(nbytes: int, nunits: int) -> engine.Batch:
 
 
 def mask_sensitive_json_bytes_batch(payloads: Sequence[bytes], max_depth: Optional[int] = None) -> List[Optional[bytes]]:
-    """Masked bytes per payload; None where the crate would raise ValueError (invalid JSON)."""
+    """Masked bytes per payload; None where the crate would raise ValueError (invalid JSON, a number out of binary64's range,
+    nesting deeper than 127 levels)."""
     if not payloads:
         return []
     depth = 10 if max_depth is None else int(max_depth)
@@ -57,7 +59,8 @@ def mask_sensitive_json_bytes_batch(payloads: Sequence[bytes], max_depth: Option
         elif st == engine.MASK_PARSE_ERROR:
             res.append(None)
         else:
-            raise RuntimeError("request_logging_masking(GPU): payload exceeds the device limits (nesting > 64 or number > 3200 bits)")
+            raise RuntimeError("request_logging_masking(GPU): payload exceeds the device limits (a number literal longer than the 3200-bit "
+                               "workspace, or a body over 768 MiB)")
     return res
 
 

@@ -231,10 +231,34 @@ def parse_serde(payload: bytes) -> Any:
     def bad(c):
         raise ValueError(c)
 
-    v = json.loads(text, parse_int=parse_int, parse_float=parse_float, parse_constant=bad)
-    if _depth(v) > 128:
+    def pairs(kv):
+        d = dict(kv)
+        if len(d) != len(kv):            # serde_json parsed the values a duplicate key overwrites as well
+            _reject_lone_surrogates([x for _, x in kv])
+        return d
+
+    v = json.loads(text, parse_int=parse_int, parse_float=parse_float, parse_constant=bad, object_pairs_hook=pairs)
+    # serde_json's check_recursion!: remaining_depth starts at 128, each '[' or '{' decrements it and the parse fails when it
+    # reaches 0, so 127 nested containers parse and 128 do not.
+    if _depth(v) > 127:
         raise ValueError("recursion limit exceeded")
+    _reject_lone_surrogates(v)
     return v
+
+
+def _reject_lone_surrogates(v: Any) -> None:
+    """json.loads keeps a \\uD800-\\uDFFF escape that is not half of a pair as a lone surrogate; serde_json rejects it while
+    parsing (parse_unicode_escape), wherever the string sits.  A valid pair has become one astral code point by now."""
+    stack = [v]
+    while stack:
+        x = stack.pop()
+        if isinstance(x, dict):
+            stack.extend(x.keys())
+            stack.extend(x.values())
+        elif isinstance(x, list):
+            stack.extend(x)
+        elif isinstance(x, str) and any("\ud800" <= c <= "\udfff" for c in x):
+            raise ValueError("lone leading or trailing surrogate in hex escape")
 
 
 def mask_json_bytes(payload: bytes, max_depth: int = 10) -> bytes:

@@ -218,6 +218,7 @@ extern "C" int cfh_toon_indexed(const uint8_t* text, uint32_t n, uint8_t* out, u
   const int pr = indexed_parse(text, n, nodes, &cnt);
   return cfj::toon_finish(pr, text, nodes.data(), out, out_cap, out_len, &big, digits.data(), (uint32_t)digits.size(), false);
 }
+// (json_build keeps the 64-level stack and has no number range check: this twin agrees with cfh_mask on bodies inside both)
 extern "C" int cfh_mask_indexed(const uint8_t* text, uint32_t n, int max_depth, uint8_t* out, uint32_t out_cap, uint32_t* out_len) {
   std::vector<cfj::JNode> nodes(n / 2 + 4);
   std::vector<uint32_t> idx(n / 2 + 4);

@@ -166,13 +166,24 @@ def json_index(data: bytes):
     return [(pos[i] & 0x7FFFFFFF, bool(pos[i] >> 31), aux[i]) for i in range(nt)], bool(unt.value)
 
 
-def mask_host(payload: bytes, max_depth: int = 10, indexed: bool = False):
-    """(status, masked_bytes_or_None) from the shared json_mask.h pipeline compiled for the CPU."""
-    cap = len(payload) * 5 + 64
-    out = ctypes.create_string_buffer(cap)
-    n = ctypes.c_uint32()
+MASK_OVERFLOW = 7
+
+
+def mask_host(payload: bytes, max_depth: int = 10, indexed: bool = False, retry: bool = True):
+    """(status, masked_bytes_or_None) from the shared json_mask.h pipeline compiled for the CPU, sized like cf_mask_host sizes a
+    unit: 5 * len + 32 bytes of room, and a unit that reports MS_OVERFLOW (7) run again into exactly the length it asked for.
+    retry=False returns the first pass as it is: (7, needed length) for a unit that outgrew its room."""
     fn = lib().cfh_mask_indexed if indexed else lib().cfh_mask
-    st = fn(payload, len(payload), max_depth, out, cap, ctypes.byref(n))
+    cap = len(payload) * 5 + 32
+    for _ in range(2):
+        out = ctypes.create_string_buffer(max(cap, 1))
+        n = ctypes.c_uint32()
+        st = fn(payload, len(payload), max_depth, out, cap, ctypes.byref(n))
+        if st != MASK_OVERFLOW or not retry:
+            break
+        cap = n.value
+    if st == MASK_OVERFLOW:
+        return st, n.value
     return st, (out.raw[: n.value] if st == 0 else None)
 
 

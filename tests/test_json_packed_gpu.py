@@ -3,8 +3,8 @@ warp for about 200, 6 000 and 40 000 units on an H100), with hostile neighbours 
 64 KiB units, nesting 63 / 64 / 65, hard numbers, escapes and surrogate pairs.  cf_mask_host (max_depth 10 and 3),
 cf_toon_host on the default path (token-parallel kernel + sequential hand-over) and with CF_TOON_SEQUENTIAL are compared
 with the oracles (oracle/mask_ref.py, oracle/toon_ref.py), never with another GPU path.  A unit beyond the documented
-device limits (nesting > 64, a number whose exact conversion needs more than 3200 bits) must report UNSUPPORTED (6)
-instead.
+device limits (a number whose exact conversion needs more than 3200 bits; for the TOON encoders also nesting > 64) must report
+UNSUPPORTED (6) instead; masking parses serde_json's 127 levels, so it holds the nested units to the oracle.
 
 A second corpus reaches every reason (json_tp.h FB_*) for which the token-parallel kernel hands a unit to the sequential
 encoder: with CF_TOON_NO_HANDOVER the reason is reported, on the default path the unit gets the oracle's answer."""
@@ -99,7 +99,7 @@ def big_json(rng, target, sensitive):
 
 
 def hostile_pool(seed):
-    """[(unit bytes, beyond the device limits?)]."""
+    """[(unit bytes, beyond the device limits?)]; "toon": beyond the TOON encoders' limits only."""
     import json
 
     rng = random.Random(seed)
@@ -108,7 +108,7 @@ def hostile_pool(seed):
             (b'"\xc3"', False), (b'{"password": "\xed\xa0\x80"}', False)]
     for kind in ("arr", "obj", "mix"):
         for d in (63, 64, 65):
-            pool.append(((nested(kind, d) + PAD).encode(), d > DEPTH_LIMIT))
+            pool.append(((nested(kind, d) + PAD).encode(), "toon" if d > DEPTH_LIMIT else False))   # masking parses serde_json's 127 levels
     pool.append(((nested("obj", 64)[:-1] + PAD).encode(), False))           # unterminated at depth 64
     for x in hard_numbers(rng):
         pool.append((('{"n": ' + x + ', "v": [' + x + ', 1], "rows": [{"a": ' + x + ', "b": 2}, {"a": 3, "b": ' + x + '}]}' + PAD).encode(), False))
@@ -212,12 +212,12 @@ def check_mask(units, md):
     st, outs = engine.mask_host(engine.Batch(ctx, len(stream), len(units)), stream, offs, md)
     bad = []
     for i, ((u, beyond), s, o) in enumerate(zip(units, st, outs)):
-        if beyond:
-            ok = s == engine.MASK_UNSUPPORTED and o is None
+        if beyond is True:          # past the workspace: UNSUPPORTED, unless the number is out of binary64's range (the crate's ValueError)
+            ok = s == (engine.MASK_PARSE_ERROR if mask_oracle(u, md) is None else engine.MASK_UNSUPPORTED) and o is None
         else:
             ok = s != engine.MASK_UNSUPPORTED and o == mask_oracle(u, md)
         if not ok:
-            bad.append((i, u[:100], int(s), (o or b"")[:100], (mask_oracle(u, md) or b"")[:100] if not beyond else "UNSUPPORTED"))
+            bad.append((i, u[:100], int(s), (o or b"")[:100], (mask_oracle(u, md) or b"")[:100] if beyond is not True else "UNSUPPORTED"))
     assert not bad, (len(bad), bad[:4])
     return st
 
@@ -247,7 +247,9 @@ def test_long_mantissas_on_the_cpu_build():
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("n", SIZES)
-def test_mask_packed_warps_vs_oracle(pool, n):
+def test_mask_packed_warps_vs_serde_limits(pool, n):
+    """Masking at serde_json's limits: the 65-level units mask like the oracle, integers beyond the 3200-bit workspace are out of
+    binary64's range (the crate's ValueError), and only in-range literals past the workspace are UNSUPPORTED."""
     units = batch_units(n, pool, n)
     for md in (10, 3):
         st = check_mask(units, md)
@@ -265,8 +267,9 @@ def test_toon_packed_warps_vs_oracle(pool, n, mode):
 
 
 @pytest.mark.gpu
-def test_every_hostile_unit_once(pool):
-    """The whole pool in one small batch (one unit per warp), so that no unit of it can escape the comparison by chance."""
+def test_every_hostile_unit_once_at_serde_limits(pool):
+    """The whole pool in one small batch (one unit per warp), so that no unit of it can escape the comparison by chance; masking
+    held to serde_json's limits as in test_mask_packed_warps_vs_serde_limits, TOON to its 64 levels."""
     check_mask(pool, 10)
     check_toon(pool, TOON_REPORT_ERRORS)
     check_toon(pool, TOON_REPORT_ERRORS | TOON_SEQUENTIAL)
