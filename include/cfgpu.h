@@ -210,9 +210,10 @@ int cf_toon_host(cf_ctx* ctx, cf_batch* b, uint32_t flags, const uint8_t* stream
  *   CF_STAGE_TOON  verdict.aux = CF_TOON_* status; CF_V_TOON when converted (out = the TOON text)
  * stream == NULL runs the stages on the batch that is ALREADY resident (uploaded by cf_batch_upload or a previous call): bench.py's
  * device-resident `value`; offsets must then be the host copy of that batch's offsets.
- *   CF_STAGE_MASK  request_logging_masking on the same upload (verdict.aux = CF_MASK_* status, out = masked JSON);
- *                  not combinable with CF_STAGE_TOON in one call (both produce the unit's output).  Rewritten texts are not
- *                  returned: a rewritten unit that does not mask keeps its rewritten length in out_len and has no output. */
+ *   CF_STAGE_MASK  request_logging_masking of every unit on the same upload (verdict.aux = CF_MASK_* status, CF_V_MASKED and
+ *                  out = the masked JSON when it masks), in cf_run_batch and cf_run_enqueue alike; not combinable with CF_STAGE_TOON
+ *                  in one call (both produce the unit's output).  Rewritten texts are not returned: a rewritten unit that does not
+ *                  mask keeps its rewritten length in out_len and has no output. */
 #define CF_STAGE_SCAN 1u
 #define CF_STAGE_SUB 2u
 #define CF_STAGE_MASK 4u
@@ -242,21 +243,23 @@ int cf_run_batch_device_output(cf_ctx* ctx, const uint8_t** d_out, uint64_t* byt
 int cf_copy_to_host(cf_ctx* ctx, void* host_dst, const void* device_src, uint64_t bytes);
 
 /* ---------------- the fused chain on the caller's stream: cf_run_enqueue / cf_run_finish ----------------
- * cf_run_batch's SCAN, SUB and TOON stages without a host round trip between launch and completion: the dirty-unit selection, the
- * substitution's scratch bounds and arena allocation, the verdict records, the output offsets and the gather are decided on the
- * device.  cf_run_batch itself is an upload, one enqueue and one finish on a run the context owns (with CF_STAGE_MASK, the masking
- * kernel after them).
+ * cf_run_batch's stages without a host round trip between launch and completion: the dirty-unit selection, the substitution's
+ * scratch bounds and arena allocation, the verdict records, the output offsets, the gather and the masking of the bodies that
+ * outgrow their first room are decided on the device.  cf_run_batch itself is an upload, one enqueue and one finish on a run the
+ * context owns.
  *
  * A cf_run owns every piece of per-call device state (scan queue, TOON scratch and unit order, the dirty-unit list, the substitution
  * descriptors and arena, per-unit gather sources, a status block, a completion event and a side stream), so runs created on one
  * ctx can be in flight at once on different streams.  Memory of a run: 8 x max_stream_bytes of TOON scratch, max_stream_bytes of
- * TOON output, about 170 bytes per unit, 8 MiB of scan queue and the arena.  (The run cf_run_batch uses borrows the context's TOON
- * workspace instead, the one cf_toon uses, so a context holds one.)
+ * TOON output, about 170 bytes per unit, 8 MiB of scan queue and the arena.  cf_run_set_mask adds the masking workspace: 7 x
+ * max_stream_bytes + 52 bytes per unit (the first pass's room of 5 len + 32 bytes per unit, and the parser's node index; its nodes
+ * are the TOON scratch).  (The run cf_run_batch uses borrows the context's TOON and masking workspaces instead, the ones cf_toon
+ * uses, so a context holds one.)
  *
  * cf_run_enqueue: the batch must be resident (cf_batch_upload on the same stream, or ordered before it).  d_verdicts (n_units
  * records), d_out_offsets (n_units + 1), d_out (out_cap bytes), d_bitmaps_full (n_units * W words; required with SCAN or SUB) and
  * d_unit_stages (may be NULL) are caller-owned DEVICE memory (torch tensors work).  Stages: CF_STAGE_SCAN, CF_STAGE_SUB (implies
- * SCAN), CF_STAGE_TOON; CF_STAGE_MASK is CF_E_BADARG (masking keeps cf_run_batch).  Results are cf_run_batch's, unit for unit.
+ * SCAN), CF_STAGE_TOON or CF_STAGE_MASK (CF_E_BADARG on a run without cf_run_set_mask).  Results are cf_run_batch's, unit for unit.
  * Between its first launch and its return the call neither synchronises, allocates nor reads device memory on the host, so it
  * can be captured in a CUDA graph.  Warm the run up with one enqueue + finish first, so that the arena has its size; a replay that
  * needs more defers the units that do not fit, and the graph stays valid: once an enqueue of a run was captured, arenas the run
@@ -266,6 +269,12 @@ int cf_copy_to_host(cf_ctx* ctx, void* host_dst, const void* device_src, uint64_
  * Deferred units: a dirty unit whose two scratch buffers (first-pass bound min(worst, 64 L + 64 KiB) each, as cf_sub_host) do not fit
  * the arena that is left, or whose rewrite outgrows that bound, gets no output in the enqueue.  cf_run_finish completes it with the
  * synchronous substitution (which regrows its room and reports CF_E_TOO_LARGE), patches its record and redoes offsets and gather.
+ *
+ * Masking: every unit masks into 5 len + 32 bytes of the run's workspace; a body whose output needs more is given its exact length in
+ * out_offsets and masked again after the gather, straight into d_out (the grid of that launch covers every unit, the few retried ones
+ * run).  A retried unit that still does not fit is an error of cf_run_finish (CF_E_CUDA).
+ * cf_run_set_mask: allocates the run's masking workspace on its first call (sized for max_units / max_stream_bytes) and sets the
+ * max_depth of the enqueues after it; later calls allocate nothing.  Call it before the enqueue that is captured.
  *
  * cf_run_finish: waits for the run's last enqueue (or a graph replay of it) and reads its status through the run's own non-blocking
  * stream (it waits for nothing else the caller has queued).  Returns CF_OK; CF_E_CAPACITY only when the gathered texts need
@@ -279,6 +288,7 @@ void cf_run_free(cf_run* run);
 int cf_run_enqueue(cf_ctx* ctx, cf_prog* prog, cf_batch* b, cf_run* run, uint32_t stage_mask, const uint8_t* d_unit_stages, uint32_t toon_flags,
                    cf_verdict* d_verdicts, uint64_t* d_bitmaps_full, uint64_t* d_out_offsets, uint8_t* d_out, uint64_t out_cap, void* cuda_stream);
 int cf_run_finish(cf_ctx* ctx, cf_run* run, uint64_t* needed);
+int cf_run_set_mask(cf_ctx* ctx, cf_run* run, int max_depth);
 
 /* number of kernels launched by this ctx so far (for bench.py's gpu_launches) */
 uint64_t cf_kernel_launches(const cf_ctx* ctx);

@@ -69,6 +69,7 @@ _SIGS = {
     "cf_run_enqueue": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_uint32, c_void_p, c_void_p, c_void_p, c_void_p, c_uint64,
                                c_void_p]),
     "cf_run_finish": (c_int, [c_void_p, c_void_p, POINTER(c_uint64)]),
+    "cf_run_set_mask": (c_int, [c_void_p, c_void_p, c_int]),
     "cf_kernel_launches": (c_uint64, [c_void_p]),
     "cf_scan_counters": (c_int, [c_void_p, c_void_p]),
     "cf_profile_begin": (c_int, [c_void_p, c_uint32]),

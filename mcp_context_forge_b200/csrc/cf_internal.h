@@ -139,9 +139,11 @@ struct RunStatus {
   int32_t err;            // CF_E_CAPACITY when the gathered texts exceed out_cap (the gather is skipped)
   uint32_t n_sel;         // dirty units the enqueue rewrites (selection list length)
   uint32_t n_deferred;    // dirty units left to cf_run_finish
-  uint32_t pad;
+  uint32_t n_retry;       // masked units that outgrew the first pass's room (retry list length)
   uint64_t needed;        // bytes of all gathered texts
   uint64_t arena_used;    // substitution arena bytes the dirty units asked for (fitting or not)
+  int32_t mask_err;       // a retried unit did not mask into the exact length its first pass asked for
+  uint32_t pad;
 };
 static const uint32_t RUN_NOT_DIRTY = 0xFFFFFFFFu;    // slot[u]: the unit is not rewritten
 static const uint32_t RUN_DEFER_PENDING = 0xFFFFFFFEu;  // ... dirty, did not fit the arena
@@ -163,7 +165,14 @@ struct cf_run {
   uint8_t* d_toon_sort = nullptr;
   size_t toon_sort_bytes = 0;
   uint8_t* d_toon_out = nullptr;                        // TOON texts in the input's layout
-  uint32_t* d_toon_ls = nullptr;                        // TOON lengths [n] | statuses [n]
+  uint32_t* d_toon_ls = nullptr;                        // TOON (or masking) lengths [n] | statuses [n]
+  // masking (cf_run_set_mask): the parser's nodes are the TOON scratch; TOON and masking never share an enqueue
+  uint8_t* d_mask_arena = nullptr;                      // first pass: unit u masks into 5 len + 32 bytes at 5 offsets[u] + 32 u
+  uint64_t mask_arena_bytes = 0;
+  uint32_t* d_mask_retry = nullptr;                     // units that outgrew their room (RunStatus::n_retry of them)
+  uint32_t* d_mask_idx = nullptr;                       // the parser's node index
+  uint64_t mask_idx_bytes = 0;
+  int mask_depth = 0;
   uint32_t* d_slot = nullptr;                           // per unit: RUN_NOT_DIRTY / selection index / RUN_DEFER*
   uint32_t* d_sel = nullptr;                            // per selection index: unit, scratch offset, bound, record
   uint64_t *d_soff = nullptr, *d_bound = nullptr, *d_rec = nullptr;
@@ -206,6 +215,7 @@ static const int CF_TS_FALLBACK = 7;                   // == cftp::TS_FALLBACK (
 static const uint32_t TOON_ONLY_FALLBACK = 0x100u;     // internal flag of toon_kernel: only units with status TS_FALLBACK
 void cf_launch_toon_seq(uint32_t blocks, cudaStream_t st, const uint8_t* stream, const uint64_t* offsets, uint32_t n_units, cfj::JNode* nodes, uint8_t* out,
                         uint32_t* out_len, int32_t* status, uint32_t flags, uint32_t upw);
-void cf_launch_mask_seq(uint32_t blocks, const uint8_t* stream, const uint64_t* offsets, uint32_t n_units, cfj::JNode* nodes, uint32_t* idx, uint8_t* out,
-                        uint32_t* out_len, int32_t* status, int max_depth, uint32_t upw, const uint32_t* retry, const uint64_t* out_off);
+void cf_launch_mask_seq(uint32_t blocks, cudaStream_t st, const uint8_t* stream, const uint64_t* offsets, uint32_t n_units, cfj::JNode* nodes, uint32_t* idx,
+                        uint8_t* out, uint32_t* out_len, int32_t* status, int max_depth, uint32_t upw, const uint32_t* retry, const uint64_t* out_off,
+                        RunStatus* rs);
 void cf_launch_classify_keys(uint32_t blocks, const uint8_t* stream, const uint64_t* offsets, uint32_t n_units, uint8_t* sensitive);

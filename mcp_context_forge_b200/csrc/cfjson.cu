@@ -272,8 +272,12 @@ struct ToonWs {
   uint8_t* sort;
   size_t sort_bytes;
 };
+// masking of a batch of nbytes / n units: the parser's nodes (in the TOON scratch, which toon_scratch_need sizes for them), the
+// first pass's arena, and the retry list | node index
+static uint64_t mask_nodes(uint64_t nbytes, uint32_t n) { return nbytes / 2 + 4ull * n + 8; }
+static uint64_t mask_arena_need(uint64_t nbytes, uint32_t n) { return 5 * nbytes + 32ull * n; }
 static uint64_t toon_scratch_need(uint64_t nbytes, uint32_t n) {
-  const uint64_t need = (nbytes / 2 + 4ull * n + 8) * sizeof(cfj::JNode);
+  const uint64_t need = mask_nodes(nbytes, n) * sizeof(cfj::JNode);      // the sequential encoder's DOM, or the mask parser's
   const uint64_t need_tp = (nbytes / 2 + (uint64_t)TP_TOK_SLACK * n + 8) * sizeof(cftp::GTok);
   return need_tp > need ? need_tp : need;
 }
@@ -435,88 +439,15 @@ int cf_toon_host(cf_ctx* ctx, cf_batch* b, uint32_t flags, const uint8_t* stream
   return CF_OK;
 }
 
-static int cf_mask_resident(cf_ctx* ctx, cf_batch* b, int max_depth, uint8_t* out_bytes, uint64_t out_cap, uint64_t* out_offsets, int32_t* status,
-                            uint64_t* out_needed);
 int cf_mask_host(cf_ctx* ctx, cf_batch* b, const uint8_t* stream, uint64_t stream_bytes, const uint64_t* offsets, uint32_t n_units,
                  int max_depth, uint8_t* out_bytes, uint64_t out_cap, uint64_t* out_offsets, int32_t* status, uint64_t* out_needed) {
   if (!ctx || !b || !out_offsets || !status) return CF_E_BADARG;
-  int rc = cf_batch_upload(ctx, b, stream, stream_bytes, offsets, n_units, nullptr);
-  if (rc) return rc;
-  return cf_mask_resident(ctx, b, max_depth, out_bytes, out_cap, out_offsets, status, out_needed);
-}
-// masking of the batch already uploaded
-static int cf_mask_resident(cf_ctx* ctx, cf_batch* b, int max_depth, uint8_t* out_bytes, uint64_t out_cap, uint64_t* out_offsets, int32_t* status,
-                            uint64_t* out_needed) {
-  int rc;
-  const uint64_t stream_bytes = b->nbytes;
-  const uint32_t n_units = b->n;
-  const uint64_t nnodes = stream_bytes / 2 + 4ull * n_units + 8;
-  const uint64_t need = nnodes * sizeof(cfj::JNode);
-  if (need > ctx->toon_scratch_bytes) {
-    cudaFree(ctx->d_toon_scratch);
-    ctx->d_toon_scratch = nullptr;
-    ctx->toon_scratch_bytes = 0;
-    CF_CUDA(ctx, cudaMalloc(&ctx->d_toon_scratch, need + need / 4));
-    ctx->toon_scratch_bytes = need + need / 4;
-  }
-  if ((rc = cf_dev_reserve(ctx, ctx->tmp[0], 5 * stream_bytes + 32ull * n_units + 64))) return rc;
-  if ((rc = cf_dev_reserve(ctx, ctx->tmp[1], (size_t)n_units * 4))) return rc;
-  if ((rc = cf_dev_reserve(ctx, ctx->tmp[2], (size_t)n_units * 4))) return rc;
-  if ((rc = cf_dev_reserve(ctx, ctx->tmp[3], ((size_t)n_units + 1) * 8))) return rc;
-  if ((rc = cf_dev_reserve(ctx, ctx->tmp[5], nnodes * 4))) return rc;
-  uint8_t* d_arena = (uint8_t*)ctx->tmp[0].p;
-  uint32_t* d_len = (uint32_t*)ctx->tmp[1].p;
-  int32_t* d_st = (int32_t*)ctx->tmp[2].p;
-  uint64_t* d_ooff = (uint64_t*)ctx->tmp[3].p;
-  uint32_t* d_idx = (uint32_t*)ctx->tmp[5].p;
-  std::vector<uint32_t> lens(n_units);
-  const uint32_t upw = units_per_warp(ctx, n_units);
-  cf_launch_mask_seq(json_blocks(n_units, upw), b->d_buf + cf::FRONT_PAD, b->d_offsets, n_units, (cfj::JNode*)ctx->d_toon_scratch, d_idx, d_arena, d_len,
-                                                 d_st, max_depth, upw, nullptr, nullptr);
-  ctx->launches++;
-  CF_CUDA(ctx, cudaGetLastError());
-  CF_CUDA(ctx, cudaMemcpy(lens.data(), d_len, (size_t)n_units * 4, cudaMemcpyDeviceToHost));
-  CF_CUDA(ctx, cudaMemcpy(status, d_st, (size_t)n_units * 4, cudaMemcpyDeviceToHost));
-  // A unit whose output outgrew its 5 * len + 32 bytes (MS_OVERFLOW, lens = the length it needs) is masked again below, straight
-  // into its place in the gathered output.  Its offsets count that length already.
-  std::vector<uint32_t> retry;
-  uint64_t total = 0;
-  for (uint32_t i = 0; i < n_units; ++i) {
-    if (status[i] == cfm::MS_OVERFLOW) retry.push_back(i);
-    out_offsets[i] = total;
-    total += lens[i];
-  }
-  out_offsets[n_units] = total;
-  if (out_needed) *out_needed = total;
-  if (total > out_cap || (!out_bytes && total)) { ctx->err = "output buffer too small"; return CF_E_CAPACITY; }
-  if (total) {
-    if ((rc = cf_dev_reserve(ctx, ctx->tmp[4], total))) return rc;
-    if ((rc = cf_stage_reserve(ctx, total))) return rc;
-    CF_CUDA(ctx, cudaMemcpy(d_ooff, out_offsets, ((size_t)n_units + 1) * 8, cudaMemcpyHostToDevice));
-    if (!retry.empty()) {        // the gather copies nothing for them (their text is not in the arena)
-      for (uint32_t u : retry) lens[u] = 0;
-      CF_CUDA(ctx, cudaMemcpy(d_len, lens.data(), (size_t)n_units * 4, cudaMemcpyHostToDevice));
-    }
-    compact_kernel<<<n_units, 128>>>(d_arena, 5, 32, b->d_offsets, d_len, d_ooff, (uint8_t*)ctx->tmp[4].p, n_units);
-    ctx->launches++;
-    CF_CUDA(ctx, cudaGetLastError());
-    if (!retry.empty()) {        // the unit list goes to the arena, which the gather has finished reading
-      const uint32_t nr = (uint32_t)retry.size();
-      uint32_t* d_retry = (uint32_t*)d_arena;
-      CF_CUDA(ctx, cudaMemcpy(d_retry, retry.data(), (size_t)nr * 4, cudaMemcpyHostToDevice));
-      const uint32_t rupw = units_per_warp(ctx, nr);
-      cf_launch_mask_seq(json_blocks(nr, rupw), b->d_buf + cf::FRONT_PAD, b->d_offsets, nr, (cfj::JNode*)ctx->d_toon_scratch, d_idx,
-                         (uint8_t*)ctx->tmp[4].p, d_len, d_st, max_depth, rupw, d_retry, d_ooff);
-      ctx->launches++;
-      CF_CUDA(ctx, cudaGetLastError());
-      CF_CUDA(ctx, cudaMemcpy(status, d_st, (size_t)n_units * 4, cudaMemcpyDeviceToHost));
-      for (uint32_t u : retry)
-        if (status[u] != cfm::MS_OK) { ctx->err = "mask_kernel: a unit retried with the room it asked for did not fit"; return CF_E_CUDA; }
-    }
-    CF_CUDA(ctx, cudaMemcpy(ctx->h_stage, ctx->tmp[4].p, total, cudaMemcpyDeviceToHost));
-    memcpy(out_bytes, ctx->h_stage, total);
-  }
-  return CF_OK;
+  std::vector<cf_verdict> v(n_units);
+  const int rc = cf_run_batch(ctx, nullptr, b, stream, stream_bytes, offsets, n_units, CF_STAGE_MASK, nullptr, 0, max_depth, v.data(), nullptr, out_bytes,
+                              out_cap, out_offsets, out_needed);
+  if (rc == CF_OK || rc == CF_E_CAPACITY)
+    for (uint32_t i = 0; i < n_units; ++i) status[i] = v[i].aux;
+  return rc;
 }
 
 int cf_classify_keys_host(cf_ctx* ctx, cf_batch* b, const uint8_t* stream, uint64_t stream_bytes, const uint64_t* offsets, uint32_t n_units,
@@ -544,12 +475,16 @@ int cf_classify_keys_host(cf_ctx* ctx, cf_batch* b, const uint8_t* stream, uint6
 // exclusive scan of len gives out_offsets[0..n]).  A dirty unit whose substitution did not run (RUN_DEFER_PENDING) or outgrew its
 // bound (SUB_OVERFLOW) is deferred: appended to `deferred`, slot[u] = RUN_DEFER | its index there, no output yet.  cf_run_finish runs
 // the kernel again with def_rec: the deferred units' records from the synchronous substitution (offsets relative to def_base).
+// With CF_STAGE_MASK, toon_ls holds the mask's first pass (lengths | statuses) and the masked bodies are the only texts gathered: a
+// unit that masked in its room gathers from the mask arena; one that outgrew it (MS_OVERFLOW, its length the exact one) is appended
+// to mask_retry and gathers nothing, the retry pass after the gather writes it in place.
 __global__ void __launch_bounds__(256) run_verdict_kernel(uint32_t n, uint32_t stage_mask, const uint8_t* __restrict__ unit_stages,
                                                           const uint64_t* __restrict__ bm, uint32_t W, const uint32_t* __restrict__ toon_ls,
                                                           uint32_t* slot, const uint64_t* __restrict__ rec, const uint8_t* arena,
                                                           const uint64_t* __restrict__ def_rec, const uint8_t* def_base, const uint8_t* stream,
-                                                          const uint64_t* __restrict__ offsets, const uint8_t* toon_out, uint32_t* __restrict__ deferred,
-                                                          RunStatus* st, cf_verdict* __restrict__ v, uint64_t* __restrict__ src, uint64_t* __restrict__ len) {
+                                                          const uint64_t* __restrict__ offsets, const uint8_t* toon_out, const uint8_t* mask_out,
+                                                          uint32_t* __restrict__ mask_retry, uint32_t* __restrict__ deferred, RunStatus* st,
+                                                          cf_verdict* __restrict__ v, uint64_t* __restrict__ src, uint64_t* __restrict__ len) {
   const uint32_t u = blockIdx.x * blockDim.x + threadIdx.x;
   if (u == n) len[n] = 0;
   if (u >= n) return;
@@ -587,6 +522,17 @@ __global__ void __launch_bounds__(256) run_verdict_kernel(uint32_t n, uint32_t s
       s = (uintptr_t)(toon_out + offsets[u]);
     }
   }
+  if (stage_mask & CF_STAGE_MASK) {                          // a rewritten unit that does not mask keeps its out_len, gathers nothing
+    aux = (int32_t)toon_ls[n + u];
+    s = 0;
+    if (aux == cfm::MS_OK || aux == cfm::MS_OVERFLOW) {
+      flags |= CF_V_MASKED;
+      out_len = toon_ls[u];
+      if (aux == cfm::MS_OK) s = (uintptr_t)(mask_out + 5 * offsets[u] + 32ull * u);
+      else mask_retry[atomicAdd(&st->n_retry, 1u)] = u;
+      aux = CF_MASK_OK;
+    }
+  }
   cf_verdict r;
   r.match_bitmap = bm ? bm[(uint64_t)u * W] : 0;
   r.flags = flags;
@@ -595,13 +541,13 @@ __global__ void __launch_bounds__(256) run_verdict_kernel(uint32_t n, uint32_t s
   r.reserved = 0;
   v[u] = r;
   src[u] = s;
-  len[u] = out_len;
+  len[u] = (stage_mask & CF_STAGE_MASK) && !(flags & CF_V_MASKED) ? 0 : out_len;
 }
 
 // gather of every produced text: dst[out_off[u], out_off[u+1]) = src[u][0, len), one warp per unit.  16-byte stores; 16-byte loads
 // when source and destination share their alignment, otherwise aligned 4-byte loads funnel-shifted into place.  Every word loaded
 // holds at least one byte of the source span, so no load leaves the span's 4-byte-aligned envelope.  When the total exceeds out_cap
-// nothing is written and the status block says so.
+// nothing is written and the status block says so.  A unit without a source (src[u] == 0) keeps its span but is not written.
 __global__ void __launch_bounds__(256) gather_kernel(const uint64_t* __restrict__ out_off, const uint64_t* __restrict__ src, uint8_t* __restrict__ out,
                                                      uint32_t n_units, uint64_t out_cap, RunStatus* st) {
   const uint32_t lane = threadIdx.x & 31;
@@ -613,8 +559,8 @@ __global__ void __launch_bounds__(256) gather_kernel(const uint64_t* __restrict_
   }
   if (total > out_cap || u >= n_units) return;
   uint64_t n = out_off[u + 1] - out_off[u];
-  if (!n) return;
   const uint8_t* s = reinterpret_cast<const uint8_t*>(src[u]);
+  if (!n || !s) return;                                      // !s: a masked unit the retry pass writes
   uint8_t* d = out + out_off[u];
   const uint64_t head = min(n, (uint64_t)((16u - ((uint32_t)(uintptr_t)d & 15u)) & 15u));
   if (lane < head) d[lane] = s[lane];
@@ -637,13 +583,21 @@ __global__ void __launch_bounds__(256) gather_kernel(const uint64_t* __restrict_
   if (lane < n - t) d[t + lane] = s[t + lane];
 }
 
-// the gather of the run's last enqueue into run->d_out (run->out_cap bytes)
+// the gather of the run's last enqueue into run->d_out (run->out_cap bytes); with CF_STAGE_MASK, then the units that outgrew the mask's
+// first pass, masked again straight into their place (the grid covers every unit: their number is only known on the device)
 static int run_gather(cf_ctx* ctx, cf_run* run) {
-  const uint32_t n = run->batch->n;
+  cf_batch* b = run->batch;
+  const uint32_t n = b->n;
   CF_CUDA(ctx, cudaMemsetAsync(&run->d_status->err, 0, sizeof(int32_t), run->st));
   gather_kernel<<<(n + 7) / 8, 256, 0, run->st>>>(run->d_out_offsets, run->d_src, run->d_out, n, run->out_cap, run->d_status);
   ctx->launches++;
   CF_CUDA(ctx, cudaGetLastError());
+  if (run->stage_mask & CF_STAGE_MASK) {
+    cf_launch_mask_seq(json_blocks(n, 1), run->st, b->d_buf + cf::FRONT_PAD, b->d_offsets, n, (cfj::JNode*)run->d_toon_scratch, run->d_mask_idx, run->d_out,
+                       run->d_toon_ls, (int32_t*)(run->d_toon_ls + n), run->mask_depth, 1, run->d_mask_retry, run->d_out_offsets, run->d_status);
+    ctx->launches++;
+    CF_CUDA(ctx, cudaGetLastError());
+  }
   return CF_OK;
 }
 
@@ -651,10 +605,11 @@ static int run_gather(cf_ctx* ctx, cf_run* run) {
 static int run_assemble(cf_ctx* ctx, cf_run* run, const uint64_t* def_rec, const uint8_t* def_base) {
   cf_batch* b = run->batch;
   const uint32_t n = b->n;
+  if (run->stage_mask & CF_STAGE_MASK) CF_CUDA(ctx, cudaMemsetAsync(&run->d_status->n_retry, 0, sizeof(uint32_t), run->st));
   run_verdict_kernel<<<(n + 256) / 256, 256, 0, run->st>>>(n, run->stage_mask, run->d_unit_stages, run->d_bitmaps, run->W, run->d_toon_ls,
                                                            run->sub ? run->d_slot : nullptr, run->d_rec, run->enq_arena, def_rec, def_base,
-                                                           b->d_buf + cf::FRONT_PAD, b->d_offsets, run->d_toon_out, run->d_deferred, run->d_status,
-                                                           run->d_verdicts, run->d_src, run->d_len);
+                                                           b->d_buf + cf::FRONT_PAD, b->d_offsets, run->d_toon_out, run->d_mask_arena, run->d_mask_retry,
+                                                           run->d_deferred, run->d_status, run->d_verdicts, run->d_src, run->d_len);
   ctx->launches++;
   CF_CUDA(ctx, cudaGetLastError());
   size_t tmp = 0;
@@ -670,6 +625,14 @@ static int run_assemble(cf_ctx* ctx, cf_run* run, const uint64_t* def_rec, const
 static int run_d2h(cf_ctx* ctx, cf_run* run, void* dst, const void* src, size_t bytes) {
   CF_CUDA(ctx, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, run->side));
   CF_CUDA(ctx, cudaStreamSynchronize(run->side));
+  return CF_OK;
+}
+
+// what the status block the run's host copy holds says of the last gather
+static int run_gather_status(cf_ctx* ctx, cf_run* run, uint64_t* needed, bool* out_short) {
+  if (run->h_status->mask_err) { ctx->err = "mask_kernel: a unit retried with the room it asked for did not fit"; return CF_E_CUDA; }
+  if (needed) *needed = run->h_status->needed;
+  if (run->h_status->err) { ctx->err = "output buffer too small"; *out_short = true; return CF_E_CAPACITY; }
   return CF_OK;
 }
 
@@ -703,9 +666,7 @@ static int run_finish(cf_ctx* ctx, cf_run* run, const uint64_t* h_offsets, uint6
     CF_CUDA(ctx, cudaStreamSynchronize(run->st));
     if ((rc = run_d2h(ctx, run, run->h_status, run->d_status, sizeof(RunStatus)))) return rc;
   }
-  if (needed) *needed = run->h_status->needed;
-  if (run->h_status->err) { ctx->err = "output buffer too small"; *out_short = true; return CF_E_CAPACITY; }
-  return CF_OK;
+  return run_gather_status(ctx, run, needed, out_short);
 }
 
 // the arena for the next call: what this one asked for, and a quarter more.  Once an enqueue of this run was captured in a CUDA graph,
@@ -791,11 +752,34 @@ void cf_run_free(cf_run* run) {
   delete run;
 }
 
+int cf_run_set_mask(cf_ctx* ctx, cf_run* run, int max_depth) {
+  if (!ctx || !run || run->ctx != ctx) return CF_E_BADARG;
+  if (!run->d_mask_arena) {             // the first call: the run's masking workspace, for its max_units / max_stream_bytes
+    if (!run->d_toon_scratch || !run->d_toon_ls) { ctx->err = "the run has no TOON scratch for the mask parser's nodes"; return CF_E_BADARG; }
+    CF_CUDA(ctx, cudaSetDevice(ctx->device));
+    const uint32_t n = run->max_units;
+    const uint64_t arena = mask_arena_need(run->max_bytes, n), idx = mask_nodes(run->max_bytes, n) * 4;
+    void *a = nullptr, *x = nullptr;
+    CF_CUDA(ctx, cudaMalloc(&a, arena));
+    run->allocs.push_back(a);
+    CF_CUDA(ctx, cudaMalloc(&x, (size_t)n * 4 + idx));
+    run->allocs.push_back(x);
+    run->d_mask_arena = (uint8_t*)a;
+    run->mask_arena_bytes = arena;
+    run->d_mask_retry = (uint32_t*)x;
+    run->d_mask_idx = (uint32_t*)x + n;
+    run->mask_idx_bytes = idx;
+  }
+  run->mask_depth = max_depth;
+  return CF_OK;
+}
+
 int cf_run_enqueue(cf_ctx* ctx, cf_prog* prog, cf_batch* b, cf_run* run, uint32_t stage_mask, const uint8_t* d_unit_stages, uint32_t toon_flags,
                    cf_verdict* d_verdicts, uint64_t* d_bitmaps_full, uint64_t* d_out_offsets, uint8_t* d_out, uint64_t out_cap, void* cuda_stream) {
   if (!ctx || !b || !run || run->ctx != ctx || !d_verdicts || !d_out_offsets || (!d_out && out_cap)) return CF_E_BADARG;
-  if (stage_mask & CF_STAGE_MASK) { ctx->err = "cf_run_enqueue runs CF_STAGE_SCAN / SUB / TOON; masking needs cf_run_batch"; return CF_E_BADARG; }
-  if (stage_mask & ~(CF_STAGE_SCAN | CF_STAGE_SUB | CF_STAGE_TOON)) { ctx->err = "unknown stage bits"; return CF_E_BADARG; }
+  if (stage_mask & ~(CF_STAGE_SCAN | CF_STAGE_SUB | CF_STAGE_MASK | CF_STAGE_TOON)) { ctx->err = "unknown stage bits"; return CF_E_BADARG; }
+  if ((stage_mask & CF_STAGE_TOON) && (stage_mask & CF_STAGE_MASK)) { ctx->err = "CF_STAGE_TOON and CF_STAGE_MASK both produce the unit's output: two calls"; return CF_E_BADARG; }
+  if ((stage_mask & CF_STAGE_MASK) && !run->d_mask_arena) { ctx->err = "CF_STAGE_MASK needs cf_run_set_mask on the run first"; return CF_E_BADARG; }
   if (stage_mask & CF_STAGE_SUB) stage_mask |= CF_STAGE_SCAN;
   if ((stage_mask & CF_STAGE_SCAN) && (!prog || !d_bitmaps_full)) { ctx->err = "CF_STAGE_SCAN / SUB need a program and d_bitmaps_full"; return CF_E_BADARG; }
   const uint32_t n = b->n;
@@ -808,6 +792,11 @@ int cf_run_enqueue(cf_ctx* ctx, cf_prog* prog, cf_batch* b, cf_run* run, uint32_
   if (stage_mask & CF_STAGE_TOON) {
     if (!run->d_toon_scratch || !run->d_toon_out) { ctx->err = "the run has no TOON workspace"; return CF_E_BADARG; }
     if ((rc = toon_ws_check(ctx, b, ws, st))) return rc;
+  }
+  if ((stage_mask & CF_STAGE_MASK) && (mask_nodes(b->nbytes, n) * sizeof(cfj::JNode) > run->toon_scratch_bytes || !run->d_toon_ls ||
+                                       mask_arena_need(b->nbytes, n) > run->mask_arena_bytes || mask_nodes(b->nbytes, n) * 4 > run->mask_idx_bytes)) {
+    ctx->err = "masking workspace too small";
+    return CF_E_CAPACITY;
   }
   size_t scan_tmp = 0;
   CF_CUDA(ctx, cub::DeviceScan::ExclusiveSum(nullptr, scan_tmp, (const uint64_t*)nullptr, (uint64_t*)nullptr, (int)n + 1, st));
@@ -840,6 +829,13 @@ int cf_run_enqueue(cf_ctx* ctx, cf_prog* prog, cf_batch* b, cf_run* run, uint32_
     if ((rc = toon_enqueue(ctx, b, toon_flags & ~(CF_TOON_PARSE_ONLY | CF_TOON_SEQUENTIAL | CF_RUN_OUTPUTS_RESIDENT), run->d_toon_out, run->d_toon_ls,
                            (int32_t*)(run->d_toon_ls + n), d_unit_stages, st, ws))) return rc;
   }
+  if (stage_mask & CF_STAGE_MASK) {     // first pass, beside the substitution: every unit into its room in the arena
+    const uint32_t upw = units_per_warp(ctx, n);
+    cf_launch_mask_seq(json_blocks(n, upw), st, b->d_buf + cf::FRONT_PAD, b->d_offsets, n, (cfj::JNode*)run->d_toon_scratch, run->d_mask_idx, run->d_mask_arena,
+                       run->d_toon_ls, (int32_t*)(run->d_toon_ls + n), run->mask_depth, upw, nullptr, nullptr, nullptr);
+    ctx->launches++;
+    CF_CUDA(ctx, cudaGetLastError());
+  }
   if (run->sub) CF_CUDA(ctx, cudaStreamWaitEvent(st, run->ev_sub, 0));
   if ((rc = run_assemble(ctx, run, nullptr, nullptr))) return rc;
   // inside a stream capture the completion event becomes a node of the graph, so that cf_run_finish waits for each replay
@@ -861,7 +857,6 @@ int cf_run_finish(cf_ctx* ctx, cf_run* run, uint64_t* needed) {
 
 // ---- the fused chain with host buffers (include/cfgpu.h): one H2D of the stream, cf_run_enqueue + cf_run_finish on the context's
 // run (legacy stream), then verdicts, offsets and only the produced texts cross PCIe back through the context's pinned staging.
-// With CF_STAGE_MASK the run (SCAN / SUB, when asked for) gives the verdicts, and the masking kernel then the texts, statuses and offsets.
 int cf_run_batch(cf_ctx* ctx, cf_prog* prog, cf_batch* b, const uint8_t* stream, uint64_t stream_bytes, const uint64_t* offsets, uint32_t n_units,
                  uint32_t stage_mask, const uint8_t* unit_stages, uint32_t toon_flags, int mask_max_depth, cf_verdict* verdicts, uint64_t* bitmaps_full,
                  uint8_t* out_bytes, uint64_t out_cap, uint64_t* out_offsets, uint64_t* out_needed) {
@@ -874,7 +869,6 @@ int cf_run_batch(cf_ctx* ctx, cf_prog* prog, cf_batch* b, const uint8_t* stream,
   // every return, error returns included, waits for the run's streams: nothing the next call's buffers are reused for stays in flight
   struct Drain { cf_ctx* c; ~Drain() { if (c->run) cudaStreamSynchronize(c->run->side); cudaStreamSynchronize(0); } } drain{ctx};
   const bool mask = (stage_mask & CF_STAGE_MASK) != 0;
-  stage_mask &= ~CF_STAGE_MASK;
   const bool keep = !mask && (toon_flags & CF_RUN_OUTPUTS_RESIDENT) != 0;
   const uint32_t W = prog ? prog->W : 1;
   int rc;
@@ -886,86 +880,86 @@ int cf_run_batch(cf_ctx* ctx, cf_prog* prog, cf_batch* b, const uint8_t* stream,
   }
   ctx->run_out = nullptr; ctx->run_out_bytes = 0;
   uint64_t total = 0;
-  bool fits = true;
-  if (mask && !stage_mask) memset(verdicts, 0, (size_t)n_units * sizeof(cf_verdict));    // masking alone: no run
-  else {
-    if (!ctx->run || ctx->run->max_units < n_units || ctx->run->max_bytes < stream_bytes) {     // the context's run, grown with the batches
-      const uint64_t arena = ctx->run ? ctx->run->arena_bytes : (1ull << 20);
-      cf_run_free(ctx->run);
-      ctx->run = nullptr;
-      if ((rc = run_create(ctx, n_units + n_units / 4, stream_bytes + stream_bytes / 4 + 4096, arena, false, &ctx->run))) return rc;
-    }
-    cf_run* run = ctx->run;
-    if (stage_mask & CF_STAGE_TOON) {       // the context's TOON workspace, lent to its run: TOON output in tmp[0], lengths | statuses in tmp[2]
-      ToonWs ws;
-      if ((rc = toon_ctx_ws(ctx, b, 0, 0, &ws)) || (rc = cf_dev_reserve(ctx, ctx->tmp[0], stream_bytes + 16)) ||
-          (rc = cf_dev_reserve(ctx, ctx->tmp[2], (size_t)n_units * 8)))
-        return rc;
-      run->d_toon_scratch = ws.scratch; run->toon_scratch_bytes = ws.scratch_bytes;
-      run->d_toon_order = ws.order; run->d_toon_sort = ws.sort; run->toon_sort_bytes = ws.sort_bytes;
-      run->d_toon_out = (uint8_t*)ctx->tmp[0].p;
-      run->d_toon_ls = (uint32_t*)ctx->tmp[2].p;
-    }
-    // pinned staging: unit_stages on the way in; verdicts | out_offsets | bitmaps on the way out
-    const size_t o_oo = ((size_t)n_units * sizeof(cf_verdict) + 15) & ~(size_t)15, o_bm = (o_oo + ((size_t)n_units + 1) * 8 + 15) & ~(size_t)15;
-    const size_t bm_bytes = (stage_mask & CF_STAGE_SCAN) ? (size_t)n_units * W * 8 : 0;
-    if ((rc = cf_stage_reserve(ctx, std::max(o_bm + bm_bytes, (size_t)n_units)))) return rc;
-    uint8_t* hs = (uint8_t*)ctx->h_stage;
-    if ((rc = cf_dev_reserve(ctx, ctx->tmp[1], (size_t)n_units * sizeof(cf_verdict))) || (rc = cf_dev_reserve(ctx, ctx->tmp[3], ((size_t)n_units + 1) * 8)) ||
-        (bm_bytes && (rc = cf_dev_reserve(ctx, ctx->tmp[6], bm_bytes))) ||
-        (rc = cf_dev_reserve(ctx, ctx->tmp[4], std::max<uint64_t>(16, keep ? stream_bytes : std::min(out_cap, stream_bytes)))))
+  if (!ctx->run || ctx->run->max_units < n_units || ctx->run->max_bytes < stream_bytes) {     // the context's run, grown with the batches
+    const uint64_t arena = ctx->run ? ctx->run->arena_bytes : (1ull << 20);
+    cf_run_free(ctx->run);
+    ctx->run = nullptr;
+    if ((rc = run_create(ctx, n_units + n_units / 4, stream_bytes + stream_bytes / 4 + 4096, arena, false, &ctx->run))) return rc;
+  }
+  cf_run* run = ctx->run;
+  if (stage_mask & CF_STAGE_TOON) {       // the context's TOON workspace, lent to its run: TOON output in tmp[0], lengths | statuses in tmp[2]
+    ToonWs ws;
+    if ((rc = toon_ctx_ws(ctx, b, 0, 0, &ws)) || (rc = cf_dev_reserve(ctx, ctx->tmp[0], stream_bytes + 16)) ||
+        (rc = cf_dev_reserve(ctx, ctx->tmp[2], (size_t)n_units * 8)))
       return rc;
-    uint8_t* d_us = nullptr;
-    if (unit_stages) {
-      if ((rc = cf_dev_reserve(ctx, ctx->tmp[7], n_units))) return rc;
-      d_us = (uint8_t*)ctx->tmp[7].p;
-      memcpy(hs, unit_stages, n_units);
-      CF_CUDA(ctx, cudaMemcpyAsync(d_us, hs, n_units, cudaMemcpyHostToDevice, 0));
-    }
-    cf_verdict* d_v = (cf_verdict*)ctx->tmp[1].p;
-    uint64_t* d_oo = (uint64_t*)ctx->tmp[3].p;
-    // the device buffer takes what the caller can take (all of it when the texts stay resident); a shortfall of the device buffer alone
-    // is made up below by growing it and gathering again.  Masking returns no rewritten texts: the run gathers none, and the
-    // CF_E_CAPACITY its finish then reports for rewritten units is expected.
-    uint8_t* d_out = mask ? nullptr : (uint8_t*)ctx->tmp[4].p;
-    const uint64_t dcap = keep ? ctx->tmp[4].cap : (d_out && out_bytes ? std::min<uint64_t>(ctx->tmp[4].cap, out_cap) : 0);
-    nvtxRangePushA("cf_run_batch:kernels");
-    rc = cf_run_enqueue(ctx, prog, b, run, stage_mask, d_us, toon_flags, d_v, bm_bytes ? (uint64_t*)ctx->tmp[6].p : nullptr, d_oo, d_out, dcap, nullptr);
-    bool out_short = false;
-    if (!rc) rc = run_finish(ctx, run, offsets, &total, &out_short);
-    nvtxRangePop();
-    if (out_short && d_out && (keep || (out_bytes && total <= out_cap))) {
-      if ((rc = cf_dev_reserve(ctx, ctx->tmp[4], total))) return rc;
-      run->d_out = (uint8_t*)ctx->tmp[4].p;
-      run->out_cap = total;
-      if ((rc = run_gather(ctx, run))) return rc;
-      CF_CUDA(ctx, cudaStreamSynchronize(0));
-    }
-    const int grown = run_grow_arena(ctx, run);
-    if (rc && !out_short) return rc;
-    if (grown) return grown;
-    Nvtx nvtx_d2h("cf_run_batch:d2h");
-    if ((rc = cf_stage_reserve(ctx, o_bm + bm_bytes))) return rc;    // a deferred unit's substitution may have grown the staging
-    hs = (uint8_t*)ctx->h_stage;
-    CF_CUDA(ctx, cudaMemcpyAsync(hs, d_v, (size_t)n_units * sizeof(cf_verdict), cudaMemcpyDeviceToHost, 0));
-    CF_CUDA(ctx, cudaMemcpyAsync(hs + o_oo, d_oo, ((size_t)n_units + 1) * 8, cudaMemcpyDeviceToHost, 0));
-    if (bitmaps_full && bm_bytes) CF_CUDA(ctx, cudaMemcpyAsync(hs + o_bm, ctx->tmp[6].p, bm_bytes, cudaMemcpyDeviceToHost, 0));
-    fits = keep || (total <= out_cap && (out_bytes || !total));
-    if (fits && d_out && !keep && total) CF_CUDA(ctx, cudaMemcpyAsync(out_bytes, ctx->tmp[4].p, total, cudaMemcpyDeviceToHost, 0));
+    run->d_toon_scratch = ws.scratch; run->toon_scratch_bytes = ws.scratch_bytes;
+    run->d_toon_order = ws.order; run->d_toon_sort = ws.sort; run->toon_sort_bytes = ws.sort_bytes;
+    run->d_toon_out = (uint8_t*)ctx->tmp[0].p;
+    run->d_toon_ls = (uint32_t*)ctx->tmp[2].p;
+  }
+  if (mask) {     // the context's buffers, lent to its run: parser nodes in the TOON scratch, arena in tmp[0], lengths | statuses in tmp[2],
+                  // retry list | node index in tmp[5]
+    ToonWs ws;
+    const uint64_t idx = mask_nodes(stream_bytes, n_units) * 4;
+    if ((rc = toon_ctx_ws(ctx, b, CF_TOON_SEQUENTIAL, 0, &ws)) || (rc = cf_dev_reserve(ctx, ctx->tmp[0], mask_arena_need(stream_bytes, n_units))) ||
+        (rc = cf_dev_reserve(ctx, ctx->tmp[2], (size_t)n_units * 8)) || (rc = cf_dev_reserve(ctx, ctx->tmp[5], (size_t)n_units * 4 + idx)))
+      return rc;
+    run->d_toon_scratch = ws.scratch; run->toon_scratch_bytes = ws.scratch_bytes;
+    run->d_toon_ls = (uint32_t*)ctx->tmp[2].p;
+    run->d_mask_arena = (uint8_t*)ctx->tmp[0].p; run->mask_arena_bytes = ctx->tmp[0].cap;
+    run->d_mask_retry = (uint32_t*)ctx->tmp[5].p; run->d_mask_idx = run->d_mask_retry + n_units; run->mask_idx_bytes = ctx->tmp[5].cap - (size_t)n_units * 4;
+    run->mask_depth = mask_max_depth;
+  }
+  // pinned staging: unit_stages on the way in; verdicts | out_offsets | bitmaps on the way out
+  const size_t o_oo = ((size_t)n_units * sizeof(cf_verdict) + 15) & ~(size_t)15, o_bm = (o_oo + ((size_t)n_units + 1) * 8 + 15) & ~(size_t)15;
+  const size_t bm_bytes = (stage_mask & CF_STAGE_SCAN) ? (size_t)n_units * W * 8 : 0;
+  if ((rc = cf_stage_reserve(ctx, std::max(o_bm + bm_bytes, (size_t)n_units)))) return rc;
+  uint8_t* hs = (uint8_t*)ctx->h_stage;
+  if ((rc = cf_dev_reserve(ctx, ctx->tmp[1], (size_t)n_units * sizeof(cf_verdict))) || (rc = cf_dev_reserve(ctx, ctx->tmp[3], ((size_t)n_units + 1) * 8)) ||
+      (bm_bytes && (rc = cf_dev_reserve(ctx, ctx->tmp[6], bm_bytes))) ||
+      (rc = cf_dev_reserve(ctx, ctx->tmp[4], std::max<uint64_t>(16, keep ? stream_bytes : std::min(out_cap, stream_bytes)))))
+    return rc;
+  uint8_t* d_us = nullptr;
+  if (unit_stages) {
+    if ((rc = cf_dev_reserve(ctx, ctx->tmp[7], n_units))) return rc;
+    d_us = (uint8_t*)ctx->tmp[7].p;
+    memcpy(hs, unit_stages, n_units);
+    CF_CUDA(ctx, cudaMemcpyAsync(d_us, hs, n_units, cudaMemcpyHostToDevice, 0));
+  }
+  cf_verdict* d_v = (cf_verdict*)ctx->tmp[1].p;
+  uint64_t* d_oo = (uint64_t*)ctx->tmp[3].p;
+  // the device buffer takes what the caller can take (all of it when the texts stay resident); a shortfall of the device buffer alone
+  // is made up below by growing it and gathering again
+  uint8_t* d_out = (uint8_t*)ctx->tmp[4].p;
+  const uint64_t dcap = keep ? ctx->tmp[4].cap : (out_bytes ? std::min<uint64_t>(ctx->tmp[4].cap, out_cap) : 0);
+  nvtxRangePushA("cf_run_batch:kernels");
+  rc = cf_run_enqueue(ctx, prog, b, run, stage_mask, d_us, toon_flags, d_v, bm_bytes ? (uint64_t*)ctx->tmp[6].p : nullptr, d_oo, d_out, dcap, nullptr);
+  bool out_short = false;
+  if (!rc) rc = run_finish(ctx, run, offsets, &total, &out_short);
+  nvtxRangePop();
+  if (out_short && (keep || (out_bytes && total <= out_cap))) {
+    if ((rc = cf_dev_reserve(ctx, ctx->tmp[4], total))) return rc;
+    run->d_out = (uint8_t*)ctx->tmp[4].p;
+    run->out_cap = total;
+    if ((rc = run_gather(ctx, run))) return rc;
     CF_CUDA(ctx, cudaStreamSynchronize(0));
-    memcpy(verdicts, hs, (size_t)n_units * sizeof(cf_verdict));
-    memcpy(out_offsets, hs + o_oo, ((size_t)n_units + 1) * 8);
-    if (bitmaps_full && bm_bytes) memcpy(bitmaps_full, hs + o_bm, bm_bytes);
+    if ((rc = run_d2h(ctx, run, run->h_status, run->d_status, sizeof(RunStatus))) || (rc = run_gather_status(ctx, run, &total, &out_short))) return rc;
   }
-  if (mask) {     // the masked bodies are the output: the mask's texts, offsets, size and CF_E_CAPACITY; its statuses patch the records
-    std::vector<int32_t> mst(n_units);
-    if ((rc = cf_mask_resident(ctx, b, mask_max_depth, out_bytes, out_cap, out_offsets, mst.data(), out_needed))) return rc;
-    for (uint32_t i = 0; i < n_units; ++i) {
-      verdicts[i].aux = mst[i];
-      if (mst[i] == CF_MASK_OK) { verdicts[i].flags |= CF_V_MASKED; verdicts[i].out_len = (uint32_t)(out_offsets[i + 1] - out_offsets[i]); }
-    }
-    return CF_OK;
-  }
+  const int grown = run_grow_arena(ctx, run);
+  if (rc && !out_short) return rc;
+  if (grown) return grown;
+  Nvtx nvtx_d2h("cf_run_batch:d2h");
+  if ((rc = cf_stage_reserve(ctx, o_bm + bm_bytes))) return rc;    // a deferred unit's substitution may have grown the staging
+  hs = (uint8_t*)ctx->h_stage;
+  CF_CUDA(ctx, cudaMemcpyAsync(hs, d_v, (size_t)n_units * sizeof(cf_verdict), cudaMemcpyDeviceToHost, 0));
+  CF_CUDA(ctx, cudaMemcpyAsync(hs + o_oo, d_oo, ((size_t)n_units + 1) * 8, cudaMemcpyDeviceToHost, 0));
+  if (bitmaps_full && bm_bytes) CF_CUDA(ctx, cudaMemcpyAsync(hs + o_bm, ctx->tmp[6].p, bm_bytes, cudaMemcpyDeviceToHost, 0));
+  const bool fits = keep || (total <= out_cap && (out_bytes || !total));
+  if (fits && !keep && total) CF_CUDA(ctx, cudaMemcpyAsync(out_bytes, ctx->tmp[4].p, total, cudaMemcpyDeviceToHost, 0));
+  CF_CUDA(ctx, cudaStreamSynchronize(0));
+  memcpy(verdicts, hs, (size_t)n_units * sizeof(cf_verdict));
+  memcpy(out_offsets, hs + o_oo, ((size_t)n_units + 1) * 8);
+  if (bitmaps_full && bm_bytes) memcpy(bitmaps_full, hs + o_bm, bm_bytes);
   if (out_needed) *out_needed = total;
   if (!fits) { ctx->err = "output buffer too small"; return CF_E_CAPACITY; }
   if (keep) {

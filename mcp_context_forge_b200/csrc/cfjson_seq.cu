@@ -37,16 +37,21 @@ __global__ void __launch_bounds__(64) toon_kernel(const uint8_t* __restrict__ st
 // request_logging_masking: mask_sensitive_json_bytes per unit (csrc/json_mask.h), plus a key classifier
 // kernel for the object-level entry points of the drop-in module.  First pass (retry == nullptr): unit u writes into its
 // 5 * len + 32 bytes at out + 5 * offsets[u] + 32 * u; a unit whose output needs more room gets MS_OVERFLOW and out_len = the
-// length it needs.  Retry pass: thread i runs unit retry[i] into exactly out_off[u + 1] - out_off[u] bytes at out + out_off[u].
+// length it needs.  Retry pass: the grid covers n_units threads, and thread i < rs->n_retry runs unit retry[i] into exactly
+// out_off[u + 1] - out_off[u] bytes at out + out_off[u]; it leaves status and out_len as the first pass wrote them and flags a unit
+// that does not fit in rs->mask_err.  Nothing runs when the gather found the output buffer too small (rs->err).
 __global__ void __launch_bounds__(64) mask_kernel(const uint8_t* __restrict__ stream, const uint64_t* __restrict__ offsets, uint32_t n_units,
                                                    cfj::JNode* __restrict__ nodes, uint32_t* __restrict__ idx, uint8_t* __restrict__ out,
                                                    uint32_t* __restrict__ out_len, int32_t* __restrict__ status, int max_depth, uint32_t upw,
-                                                   const uint32_t* __restrict__ retry, const uint64_t* __restrict__ out_off) {
+                                                   const uint32_t* __restrict__ retry, const uint64_t* __restrict__ out_off, RunStatus* rs) {
   const uint32_t lane = threadIdx.x & 31;
   if (lane >= upw) return;
   uint32_t u = ((blockIdx.x * blockDim.x + threadIdx.x) >> 5) * upw + lane;
   if (u >= n_units) return;
-  if (retry) u = retry[u];
+  if (retry) {
+    if (u >= rs->n_retry || rs->err) return;
+    u = retry[u];
+  }
   const uint64_t b = offsets[u];
   const uint64_t len64 = offsets[u + 1] - b - 1;
   if (len64 > 0x30000000ull) { status[u] = cfm::MS_UNSUPPORTED; out_len[u] = 0; return; }
@@ -60,6 +65,10 @@ __global__ void __launch_bounds__(64) mask_kernel(const uint8_t* __restrict__ st
   const uint32_t cap = retry ? (uint32_t)(out_off[u + 1] - out_off[u]) : 5 * len + 32;
   uint32_t ol = 0;
   const int st = cfm::mask_process(stream + b, len, my, len / 2 + 4, myidx, len / 2 + 4, dst, cap, &ol, max_depth, w);
+  if (retry) {
+    if (st != cfm::MS_OK) rs->mask_err = 1;
+    return;
+  }
   status[u] = st;
   out_len[u] = st == cfm::MS_OK || st == cfm::MS_OVERFLOW ? ol : 0;
 }
@@ -77,9 +86,10 @@ void cf_launch_toon_seq(uint32_t blocks, cudaStream_t st, const uint8_t* stream,
                         uint32_t* out_len, int32_t* status, uint32_t flags, uint32_t upw) {
   toon_kernel<<<blocks, 64, 0, st>>>(stream, offsets, n_units, nodes, out, out_len, status, flags, upw);
 }
-void cf_launch_mask_seq(uint32_t blocks, const uint8_t* stream, const uint64_t* offsets, uint32_t n_units, cfj::JNode* nodes, uint32_t* idx, uint8_t* out,
-                        uint32_t* out_len, int32_t* status, int max_depth, uint32_t upw, const uint32_t* retry, const uint64_t* out_off) {
-  mask_kernel<<<blocks, 64>>>(stream, offsets, n_units, nodes, idx, out, out_len, status, max_depth, upw, retry, out_off);
+void cf_launch_mask_seq(uint32_t blocks, cudaStream_t st, const uint8_t* stream, const uint64_t* offsets, uint32_t n_units, cfj::JNode* nodes, uint32_t* idx,
+                        uint8_t* out, uint32_t* out_len, int32_t* status, int max_depth, uint32_t upw, const uint32_t* retry, const uint64_t* out_off,
+                        RunStatus* rs) {
+  mask_kernel<<<blocks, 64, 0, st>>>(stream, offsets, n_units, nodes, idx, out, out_len, status, max_depth, upw, retry, out_off, rs);
 }
 void cf_launch_classify_keys(uint32_t blocks, const uint8_t* stream, const uint64_t* offsets, uint32_t n_units, uint8_t* sensitive) {
   classify_keys_kernel<<<blocks, 128>>>(stream, offsets, n_units, sensitive);

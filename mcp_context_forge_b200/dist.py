@@ -88,7 +88,7 @@ class ShardedChain:
     def partition(self, sizes: Sequence[int]) -> List[List[int]]:
         return partition_units(sizes, self.world)
 
-    def _local(self, units, stage_mask: int, unit_stages, toon_flags: int):
+    def _local(self, units, stage_mask: int, unit_stages, toon_flags: int, mask_max_depth: int = 10):
         """This rank's shard through the fused chain (GPU).  Overridable: the gloo CPU test substitutes the oracle here."""
         engine = self.engine
         if self.ctx is None:
@@ -100,10 +100,10 @@ class ShardedChain:
         b = self.batch
         if b is None or len(stream) > b.max_bytes or len(enc) > b.max_units:
             self.batch = b = engine.Batch(self.ctx, max(len(stream) * 2, 1 << 20), max(len(enc) * 2, 1024))
-        v, out, oo, _ = engine.run_batch(self.prog, b, stream, offs, stage_mask, unit_stages, toon_flags)
+        v, out, oo, _ = engine.run_batch(self.prog, b, stream, offs, stage_mask, unit_stages, toon_flags, mask_max_depth)
         return v, out, oo
 
-    def _enqueue_device(self, units, stage_mask: int, unit_stages, toon_flags: int, words: int):
+    def _enqueue_device(self, units, stage_mask: int, unit_stages, toon_flags: int, words: int, mask_max_depth: int = 10):
         """NCCL: this rank's shard through cf_run_enqueue on the current stream, verdict records left in device memory (int64 words)
         for the collective.  Returns (records, finish), finish() -> (out, out_offsets) on the host once the chain is done."""
         import torch
@@ -129,11 +129,11 @@ class ShardedChain:
         state = {"out": torch.empty(max(len(stream), 16), dtype=torch.uint8, device=dev)}
 
         def enqueue():
-            self.run_dev.enqueue(self.prog, b, stage_mask, d_us, toon_flags, d_v, d_oo, state["out"], stream=cs)
+            self.run_dev.enqueue(self.prog, b, stage_mask, d_us, toon_flags, d_v, d_oo, state["out"], stream=cs, mask_max_depth=mask_max_depth)
 
         def finish():
             need = self.run_dev.finish()
-            if need:                                      # rewritten texts outgrew the input's size: once more with the room they need
+            if need:                                      # rewritten or masked texts outgrew the input's size: once more with the room they need
                 state["out"] = torch.empty(need, dtype=torch.uint8, device=dev)
                 enqueue()
                 self.run_dev.finish()
@@ -143,7 +143,7 @@ class ShardedChain:
         enqueue()
         return d_v, finish
 
-    def run(self, units: Sequence, parts: List[List[int]], stage_mask: int, unit_stages=None, toon_flags: int = 0):
+    def run(self, units: Sequence, parts: List[List[int]], stage_mask: int, unit_stages=None, toon_flags: int = 0, mask_max_depth: int = 10):
         import torch
         import torch.distributed as dist
 
@@ -154,13 +154,15 @@ class ShardedChain:
         us = None if unit_stages is None or not mine else np.asarray(unit_stages, dtype=np.uint8)[mine]
         # NCCL with the GPU chain: verdict records stay on the device, the all-gather runs on the chain's stream, the host copy comes
         # after the collective
-        on_device = bool(mine) and self.backend == "nccl" and type(self)._local is ShardedChain._local and not stage_mask & CF_STAGE_MASK
+        on_device = bool(mine) and self.backend == "nccl" and type(self)._local is ShardedChain._local
         finish = None
         if on_device:
-            local, finish = self._enqueue_device([units[i] for i in mine], stage_mask, us, toon_flags, words)
+            local, finish = self._enqueue_device([units[i] for i in mine], stage_mask, us, toon_flags, words, mask_max_depth)
         else:
             if mine:
-                v, out, oo = self._local([units[i] for i in mine], stage_mask, us, toon_flags)
+                # the depth only when masking is asked for, so that an override of _local without masking keeps its signature
+                depth = {"mask_max_depth": mask_max_depth} if stage_mask & CF_STAGE_MASK else {}
+                v, out, oo = self._local([units[i] for i in mine], stage_mask, us, toon_flags, **depth)
             else:
                 v, out, oo = np.zeros(0, dtype=self.engine.VERDICT_DTYPE), np.zeros(0, dtype=np.uint8), np.zeros(1, dtype=np.uint64)
             local = torch.from_numpy(np.ascontiguousarray(v).view(np.int64).copy()).to(dev)

@@ -325,7 +325,7 @@ def _dev_ptr(x) -> Optional[int]:
 
 
 class Run:
-    """cf_run: the fused chain (scan, regex_filter rewriting, TOON) enqueued on the caller's CUDA stream, with verdicts, offsets and
+    """cf_run: the fused chain (scan, regex_filter rewriting, TOON or masking) enqueued on the caller's CUDA stream, with verdicts, offsets and
     texts left in device memory.  `enqueue` returns as soon as the work is queued (it may be captured in a CUDA graph); `finish`
     waits for it.  Each Run holds its own device state, so several can be in flight on different streams.
 
@@ -343,11 +343,13 @@ class Run:
         self._keep = ()
 
     def enqueue(self, prog: Optional[Program], batch: Batch, stage_mask: int, d_unit_stages, toon_flags: int, verdicts, out_offsets, out,
-                bitmaps_full=None, stream=0) -> None:
+                bitmaps_full=None, stream=0, mask_max_depth: int = 10) -> None:
         """verdicts: n * 24 bytes (e.g. a uint8 / int64 tensor), out_offsets: n + 1 uint64, out: the texts' buffer (its byte size is
         the capacity), bitmaps_full: n * W uint64 (allocated here when None and SCAN / SUB run).  Tensor sizes are checked against
         the batch (ValueError); raw device pointers are taken as they are.  `stream`: a torch.cuda.Stream or a raw
-        cudaStream_t.  The buffers must stay alive and untouched until finish()."""
+        cudaStream_t.  The buffers must stay alive and untouched until finish().
+        With CF_STAGE_MASK the bodies are masked at `mask_max_depth`; the first masking enqueue of a Run allocates its masking
+        workspace, so it must not be the one captured in a CUDA graph (warm the Run up with one enqueue + finish first)."""
         n = int(self.ctx.lib.cf_batch_units(batch.h))
         scan = bool(stage_mask & (N.CF_STAGE_SCAN | N.CF_STAGE_SUB))
         if bitmaps_full is None and scan:
@@ -366,6 +368,8 @@ class Run:
         st = getattr(stream, "cuda_stream", stream)
         self._keep = (verdicts, out_offsets, out, bitmaps_full, d_unit_stages)
         with self.ctx.lock:
+            if stage_mask & N.CF_STAGE_MASK:
+                self.ctx.check(self.ctx.lib.cf_run_set_mask(self.ctx.h, self.h, mask_max_depth), "cf_run_set_mask")
             self.ctx.check(self.ctx.lib.cf_run_enqueue(self.ctx.h, prog.h if prog is not None else None, batch.h, self.h, stage_mask, _dev_ptr(d_unit_stages),
                                                        toon_flags, _dev_ptr(verdicts), _dev_ptr(bitmaps_full), _dev_ptr(out_offsets), _dev_ptr(out), cap,
                                                        st or None), "cf_run_enqueue")
