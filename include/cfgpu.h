@@ -114,6 +114,19 @@ void cf_batch_free(cf_batch* b);
 /* async H2D of a packed stream on `cuda_stream` (cudaStream_t, may be NULL) */
 int cf_batch_upload(cf_ctx* ctx, cf_batch* b, const uint8_t* stream, uint64_t stream_bytes,
                     const uint64_t* offsets, uint32_t n_units, void* cuda_stream);
+/* Fill batch b from DEVICE memory on `cuda_stream`: unit i = d_src[d_src_offsets[i] .. d_src_offsets[i+1]), i < n_units (the
+ * offsets are absolute positions in d_src, so d_src_offsets[0] need not be 0; a run's d_out / d_out_offsets qualify as they are).
+ * src_bytes = d_src_offsets[n] - d_src_offsets[0], stated by the caller: the host never reads device memory here.
+ * The batch then holds src_bytes + n_units stream bytes, exactly as cf_batch_upload of the same units would leave it: the packed
+ * stream with its 0xFF terminators, offsets[i] = d_src_offsets[i] - d_src_offsets[0] + i, the coarse unit index and the tail padding
+ * are all built on the device, and every consumer of the batch (cf_scan, cf_toon, cf_json_index, cf_run_enqueue, cf_sub_host) sees
+ * no difference.  CF_E_BADARG for a NULL pointer or n_units == 0, CF_E_CAPACITY when src_bytes + n_units or n_units exceed the
+ * batch; both are returned before anything is queued.  Offsets that are not monotone, or a src_bytes that does not match them, give
+ * wrong units but no write outside the batch; d_src must hold every byte the offsets name.  Between its first launch and its return
+ * the call neither synchronises, allocates nor reads device memory on the host, so it can be captured in a CUDA graph together with
+ * a cf_run_enqueue of the batch.  The source must stay untouched until the work queued on `cuda_stream` has run. */
+int cf_batch_pack_device(cf_ctx* ctx, cf_batch* b, const uint8_t* d_src, const uint64_t* d_src_offsets, uint32_t n_units,
+                         uint64_t src_bytes, void* cuda_stream);
 uint32_t cf_batch_units(const cf_batch* b);
 uint64_t cf_batch_bytes(const cf_batch* b);
 /* Page-locked host memory for the buffers a caller hands to the *_host / cf_run_batch entry points (packed stream in, produced
@@ -206,7 +219,10 @@ int cf_toon_host(cf_ctx* ctx, cf_batch* b, uint32_t flags, const uint8_t* stream
  *   CF_STAGE_SCAN  verdict.match_bitmap = word 0 of the unit's pattern bitmap (all W words in bitmaps_full when not NULL)
  *   CF_STAGE_SUB   units with a set CF_PAT_ORDERED bit are rewritten rule after rule (cf_sub_host semantics): CF_V_REWRITTEN.
  *                  Such a unit is NOT TOON-encoded in the same call (the reference would encode the rewritten text): the
- *                  caller re-submits it; flags carry CF_V_RESUBMIT when TOON was requested for it.
+ *                  caller re-submits it; flags carry CF_V_RESUBMIT when TOON was requested for it.  On the device, after
+ *                  cf_run_finish returned *needed: cf_batch_pack_device(ctx, b2, d_out, d_out_offsets, n_units, needed, stream),
+ *                  d_unit_stages[i] = (flags & CF_V_RESUBMIT) ? CF_STAGE_TOON : 0 computed from the verdicts, and a
+ *                  CF_STAGE_TOON enqueue over b2 (every other unit reports CF_TOON_SKIPPED); all of it graph-capturable.
  *   CF_STAGE_TOON  verdict.aux = CF_TOON_* status; CF_V_TOON when converted (out = the TOON text)
  * stream == NULL runs the stages on the batch that is ALREADY resident (uploaded by cf_batch_upload or a previous call): bench.py's
  * device-resident `value`; offsets must then be the host copy of that batch's offsets.

@@ -51,6 +51,7 @@ _SIGS = {
     "cf_host_alloc": (c_int, [c_void_p, c_uint64, POINTER(c_void_p)]),
     "cf_host_free": (None, [c_void_p, c_void_p]),
     "cf_batch_upload": (c_int, [c_void_p, c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p]),
+    "cf_batch_pack_device": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_uint64, c_void_p]),
     "cf_batch_units": (c_uint32, [c_void_p]),
     "cf_batch_bytes": (c_uint64, [c_void_p]),
     "cf_scan": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),

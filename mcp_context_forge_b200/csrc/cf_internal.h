@@ -97,7 +97,7 @@ struct cf_batch {
   cf_ctx* ctx = nullptr;
   uint8_t* d_buf = nullptr;        // FRONT_PAD + stream + tail pad
   uint64_t* d_offsets = nullptr;
-  uint32_t* d_coarse = nullptr;    // unit index at every 4 KiB of stream (built on upload)
+  uint32_t* d_coarse = nullptr;    // unit index at every 4 KiB of stream (built on upload, or on the device by a pack)
   std::vector<uint32_t> h_coarse;
   uint64_t cap_bytes = 0;
   uint32_t cap_units = 0;
@@ -203,6 +203,33 @@ struct cf_run {
   uint8_t* d_out = nullptr;
   uint64_t out_cap = 0;
 };
+
+// out[at, at + n) = s[0, n) by the 32 lanes of one warp (gather_kernel, pack_copy_kernel).  16-byte stores; 16-byte loads when source
+// and destination share their alignment, otherwise aligned 4-byte loads funnel-shifted into place.  Every word loaded holds at least
+// one byte of the source span, so no load leaves the span's 4-byte-aligned envelope; every store stays inside out[at, at + n).
+// (The destination is passed as base and offset: that way gather_kernel compiles to the same SASS as with the copy written inline.)
+__device__ __forceinline__ void warp_copy_span(uint8_t* out, uint64_t at, const uint8_t* s, uint64_t n, uint32_t lane) {
+  uint8_t* d = out + at;
+  const uint64_t head = min(n, (uint64_t)((16u - ((uint32_t)(uintptr_t)d & 15u)) & 15u));
+  if (lane < head) d[lane] = s[lane];
+  d += head; s += head; n -= head;
+  const uint64_t nv = n >> 4;
+  uint4* dv = reinterpret_cast<uint4*>(d);
+  if (((uint32_t)(uintptr_t)s & 15u) == 0) {
+    const uint4* sv = reinterpret_cast<const uint4*>(s);
+    for (uint64_t k = lane; k < nv; k += 32) dv[k] = sv[k];
+  } else {
+    const uint32_t* sw = reinterpret_cast<const uint32_t*>((uintptr_t)s & ~(uintptr_t)3);
+    const uint32_t sh = ((uint32_t)(uintptr_t)s & 3u) * 8u;
+    for (uint64_t k = lane; k < nv; k += 32) {
+      const uint32_t* q = sw + 4 * k;
+      const uint32_t w0 = q[0], w1 = q[1], w2 = q[2], w3 = q[3], w4 = sh ? q[4] : 0u;
+      dv[k] = make_uint4(__funnelshift_r(w0, w1, sh), __funnelshift_r(w1, w2, sh), __funnelshift_r(w2, w3, sh), __funnelshift_r(w3, w4, sh));
+    }
+  }
+  const uint64_t t = nv << 4;
+  if (lane < n - t) d[t + lane] = s[t + lane];
+}
 
 // the scan of cf_scan on a given candidate queue / counter pair (cfgpu.cu)
 int cf_scan_launch(cf_ctx* ctx, cf_prog* p, cf_batch* b, uint64_t* d_bitmaps, cudaStream_t st, uint64_t* queue, uint64_t* qstate, uint32_t* qphase);

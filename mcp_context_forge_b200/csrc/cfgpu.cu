@@ -121,7 +121,7 @@ struct ScanParams {
   uint64_t nbytes;           // stream length including terminators
   uint64_t ntiles;
   const uint64_t* offsets;
-  const uint32_t* coarse;    // coarse[k] = unit containing stream byte k << COARSE_SHIFT
+  const uint32_t* coarse;    // coarse[k] = unit containing stream byte k << cf::COARSE_SHIFT
   uint32_t n_units;
   const uint32_t* E;
   cf::DfaTables dfa;
@@ -138,9 +138,8 @@ struct ScanParams {
 // Verify one candidate start: run the anchored class DFA from `start` until it dies or reaches the
 // unit's 0xFF terminator; unit boundaries come from the terminators themselves.  The unit INDEX is
 // only needed when something matched: one probe of the 4 KiB-granular coarse index + a short walk.
-static const uint32_t COARSE_SHIFT = 12;
 __device__ __forceinline__ uint32_t unit_of(const ScanParams& P, uint64_t pos) {
-  uint32_t u = P.coarse[pos >> COARSE_SHIFT];
+  uint32_t u = P.coarse[pos >> cf::COARSE_SHIFT];
   while (P.offsets[u + 1] <= pos) ++u;
   return u;
 }
@@ -1116,7 +1115,7 @@ int cf_batch_create(cf_ctx* ctx, uint64_t max_stream_bytes, uint32_t max_units, 
   CF_CUDA(ctx, cudaMalloc(&b->d_buf, total));
   CF_CUDA(ctx, cudaMemset(b->d_buf, 0xFF, total));
   CF_CUDA(ctx, cudaMalloc(&b->d_offsets, ((uint64_t)max_units + 1) * 8));
-  CF_CUDA(ctx, cudaMalloc(&b->d_coarse, ((max_stream_bytes >> COARSE_SHIFT) + 2) * 4));
+  CF_CUDA(ctx, cudaMalloc(&b->d_coarse, ((max_stream_bytes >> cf::COARSE_SHIFT) + 2) * 4));
   // tensor map for the scan kernel's tile loads
   typedef CUresult (*encode_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                 const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -1160,6 +1159,12 @@ void cf_batch_free(cf_batch* b) {
 uint32_t cf_batch_units(const cf_batch* b) { return b ? b->n : 0; }
 uint64_t cf_batch_bytes(const cf_batch* b) { return b ? b->nbytes : 0; }
 
+// cf_batch::generation of a batch's new contents (cf_batch_upload, cf_batch_pack_device)
+static uint64_t next_batch_generation() {
+  static std::atomic<uint64_t> serial{0};
+  return ++serial;
+}
+
 int cf_batch_upload(cf_ctx* ctx, cf_batch* b, const uint8_t* stream, uint64_t stream_bytes,
                     const uint64_t* offsets, uint32_t n_units, void* cuda_stream) {
   if (!ctx || !b || !stream || !offsets || !n_units) return CF_E_BADARG;
@@ -1171,11 +1176,11 @@ int cf_batch_upload(cf_ctx* ctx, cf_batch* b, const uint8_t* stream, uint64_t st
   // would otherwise queue behind the big one), then the stream itself
   CF_CUDA(ctx, cudaMemcpyAsync(b->d_offsets, offsets, ((uint64_t)n_units + 1) * 8, cudaMemcpyHostToDevice, st));
   {  // coarse unit index (host sweep over offsets; tiny next to the stream copy)
-    const uint64_t nc = (stream_bytes >> COARSE_SHIFT) + 1;
+    const uint64_t nc = (stream_bytes >> cf::COARSE_SHIFT) + 1;
     b->h_coarse.resize(nc);
     uint32_t u = 0;
     for (uint64_t k = 0; k < nc; ++k) {
-      const uint64_t pos = k << COARSE_SHIFT;
+      const uint64_t pos = k << cf::COARSE_SHIFT;
       while (u + 1 < n_units && offsets[u + 1] <= pos) ++u;
       b->h_coarse[k] = u;
     }
@@ -1187,8 +1192,53 @@ int cf_batch_upload(cf_ctx* ctx, cf_batch* b, const uint8_t* stream, uint64_t st
   CF_CUDA(ctx, cudaMemcpyAsync(d_stream, stream, stream_bytes, cudaMemcpyHostToDevice, st));
   b->nbytes = stream_bytes;
   b->n = n_units;
-  static std::atomic<uint64_t> upload_serial{0};
-  b->generation = ++upload_serial;
+  b->generation = next_batch_generation();
+  return CF_OK;
+}
+}  // extern "C"
+
+// cf_batch_pack_device: offsets[i] (i <= n) and coarse[k] (k < nc) of the packed batch, one thread per entry, from the source offsets
+__global__ void __launch_bounds__(256) pack_index_kernel(const uint64_t* __restrict__ src_off, uint32_t n, uint64_t nbytes, uint64_t nc,
+                                                         uint64_t* __restrict__ offsets, uint32_t* __restrict__ coarse) {
+  const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t <= n) offsets[t] = cf::packed_offset(src_off, (uint32_t)t, nbytes);
+  if (t < nc) coarse[t] = cf::packed_coarse(src_off, n, nbytes, t);
+}
+
+// ... and the stream: unit i's bytes and its terminator, one warp per unit.  Every write is clamped to stream[0, nbytes).
+__global__ void __launch_bounds__(256) pack_copy_kernel(const uint8_t* __restrict__ src, const uint64_t* __restrict__ src_off, uint32_t n,
+                                                        uint64_t nbytes, uint8_t* __restrict__ stream) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t u = (uint32_t)(((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  if (u >= n) return;
+  const uint64_t at = cf::packed_offset(src_off, u, nbytes);
+  const uint64_t len = min(src_off[u + 1] - src_off[u], nbytes - at);
+  warp_copy_span(stream, at, src + src_off[u], len, lane);
+  if (lane == 0 && at + len < nbytes) stream[at + len] = cf::TERM;
+}
+
+extern "C" {
+int cf_batch_pack_device(cf_ctx* ctx, cf_batch* b, const uint8_t* d_src, const uint64_t* d_src_offsets, uint32_t n_units, uint64_t src_bytes,
+                         void* cuda_stream) {
+  if (!ctx || !b || !d_src || !d_src_offsets || !n_units) return CF_E_BADARG;
+  if (n_units > b->cap_units || src_bytes > b->cap_bytes || src_bytes + n_units > b->cap_bytes) { ctx->err = "batch capacity exceeded"; return CF_E_CAPACITY; }
+  cudaStream_t st = (cudaStream_t)cuda_stream;
+  const uint64_t nbytes = src_bytes + n_units;
+  const uint64_t nc = (nbytes >> cf::COARSE_SHIFT) + 1;
+  uint8_t* d_stream = b->d_buf + cf::FRONT_PAD;
+  // the tail padding, as cf_batch_upload re-arms it; the kernels write nothing at or past nbytes
+  const uint64_t end = (ntiles_for(b->nbytes > nbytes ? b->nbytes : nbytes, MAX_TILE) + 1) * (uint64_t)MAX_TILE;
+  CF_CUDA(ctx, cudaMemsetAsync(d_stream + nbytes, 0xFF, end - nbytes, st));
+  const uint64_t idx_threads = nc > (uint64_t)n_units + 1 ? nc : (uint64_t)n_units + 1;
+  pack_index_kernel<<<(unsigned)((idx_threads + 255) / 256), 256, 0, st>>>(d_src_offsets, n_units, nbytes, nc, b->d_offsets, b->d_coarse);
+  ctx->launches++;
+  CF_CUDA(ctx, cudaGetLastError());
+  pack_copy_kernel<<<(n_units + 7) / 8, 256, 0, st>>>(d_src, d_src_offsets, n_units, nbytes, d_stream);
+  ctx->launches++;
+  CF_CUDA(ctx, cudaGetLastError());
+  b->nbytes = nbytes;
+  b->n = n_units;
+  b->generation = next_batch_generation();
   return CF_OK;
 }
 

@@ -544,10 +544,9 @@ __global__ void __launch_bounds__(256) run_verdict_kernel(uint32_t n, uint32_t s
   len[u] = (stage_mask & CF_STAGE_MASK) && !(flags & CF_V_MASKED) ? 0 : out_len;
 }
 
-// gather of every produced text: dst[out_off[u], out_off[u+1]) = src[u][0, len), one warp per unit.  16-byte stores; 16-byte loads
-// when source and destination share their alignment, otherwise aligned 4-byte loads funnel-shifted into place.  Every word loaded
-// holds at least one byte of the source span, so no load leaves the span's 4-byte-aligned envelope.  When the total exceeds out_cap
-// nothing is written and the status block says so.  A unit without a source (src[u] == 0) keeps its span but is not written.
+// gather of every produced text: dst[out_off[u], out_off[u+1]) = src[u][0, len), one warp per unit (warp_copy_span).  When the total
+// exceeds out_cap nothing is written and the status block says so.  A unit without a source (src[u] == 0) keeps its span but is not
+// written.
 __global__ void __launch_bounds__(256) gather_kernel(const uint64_t* __restrict__ out_off, const uint64_t* __restrict__ src, uint8_t* __restrict__ out,
                                                      uint32_t n_units, uint64_t out_cap, RunStatus* st) {
   const uint32_t lane = threadIdx.x & 31;
@@ -561,26 +560,7 @@ __global__ void __launch_bounds__(256) gather_kernel(const uint64_t* __restrict_
   uint64_t n = out_off[u + 1] - out_off[u];
   const uint8_t* s = reinterpret_cast<const uint8_t*>(src[u]);
   if (!n || !s) return;                                      // !s: a masked unit the retry pass writes
-  uint8_t* d = out + out_off[u];
-  const uint64_t head = min(n, (uint64_t)((16u - ((uint32_t)(uintptr_t)d & 15u)) & 15u));
-  if (lane < head) d[lane] = s[lane];
-  d += head; s += head; n -= head;
-  const uint64_t nv = n >> 4;
-  uint4* dv = reinterpret_cast<uint4*>(d);
-  if (((uint32_t)(uintptr_t)s & 15u) == 0) {
-    const uint4* sv = reinterpret_cast<const uint4*>(s);
-    for (uint64_t k = lane; k < nv; k += 32) dv[k] = sv[k];
-  } else {
-    const uint32_t* sw = reinterpret_cast<const uint32_t*>((uintptr_t)s & ~(uintptr_t)3);
-    const uint32_t sh = ((uint32_t)(uintptr_t)s & 3u) * 8u;
-    for (uint64_t k = lane; k < nv; k += 32) {
-      const uint32_t* q = sw + 4 * k;
-      const uint32_t w0 = q[0], w1 = q[1], w2 = q[2], w3 = q[3], w4 = sh ? q[4] : 0u;
-      dv[k] = make_uint4(__funnelshift_r(w0, w1, sh), __funnelshift_r(w1, w2, sh), __funnelshift_r(w2, w3, sh), __funnelshift_r(w3, w4, sh));
-    }
-  }
-  const uint64_t t = nv << 4;
-  if (lane < n - t) d[t + lane] = s[t + lane];
+  warp_copy_span(out, out_off[u], s, n, lane);
 }
 
 // the gather of the run's last enqueue into run->d_out (run->out_cap bytes); with CF_STAGE_MASK, then the units that outgrew the mask's

@@ -30,6 +30,29 @@ namespace cf {
 static const uint8_t  TERM      = 0xFF;
 static const uint32_t FRONT_PAD = 256;
 
+// Coarse unit index of a batch: coarse[k] = the unit that holds stream byte k << COARSE_SHIFT, for k in [0, nbytes >> COARSE_SHIFT].
+static const uint32_t COARSE_SHIFT = 12;
+
+// A batch packed from device memory (cf_batch_pack_device): unit i is src[src_off[i] .. src_off[i+1]) of the source, and starts in the
+// stream at its source offset rebased to unit 0 plus one terminator per unit before it.  Clamped to the stream's `nbytes`, so that
+// offsets that are not monotone give wrong units but never a position past the stream.
+CF_HD uint64_t packed_offset(const uint64_t* src_off, uint32_t i, uint64_t nbytes) {
+  const uint64_t o = src_off[i] - src_off[0] + i;
+  return o < nbytes ? o : nbytes;
+}
+// coarse[k] of that batch: the last unit i in [0, n) whose packed offset is <= k << COARSE_SHIFT (an upper-bound binary search over
+// units 1 .. n-1), which is what cf_batch_upload's host sweep finds for monotone offsets.  Always in [0, n).
+CF_HD uint32_t packed_coarse(const uint64_t* src_off, uint32_t n, uint64_t nbytes, uint64_t k) {
+  const uint64_t pos = k << COARSE_SHIFT;
+  uint32_t lo = 1, hi = n;   // the first unit in [1, n) that starts after pos, or n
+  while (lo < hi) {
+    const uint32_t mid = lo + (hi - lo) / 2;
+    if (packed_offset(src_off, mid, nbytes) <= pos) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo - 1;
+}
+
 // previous-character contexts (needed by \b, \B, ^, \A)
 enum : uint32_t { P_START = 0, P_WORD = 1, P_NL = 2, P_OTHER = 3 };
 

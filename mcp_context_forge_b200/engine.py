@@ -185,6 +185,51 @@ class Batch:
         with self.ctx.lock:
             self.ctx.check(self.ctx.lib.cf_batch_upload(self.ctx.h, self.h, sp, nbytes, offsets.ctypes.data, n, cuda_stream), "cf_batch_upload")
 
+    def pack_device(self, src, offsets, n: Optional[int] = None, stream=0, src_bytes: Optional[int] = None) -> None:
+        """cf_batch_pack_device: fill the batch from texts already in device memory, unit i = src[offsets[i] .. offsets[i+1]), with
+        the result cf_batch_upload of the same units would give.  A Run's `out` / `out_offsets` can be packed as they are, with
+        src_bytes=run.gathered_bytes.
+
+        src: a contiguous CUDA uint8 tensor or a raw device pointer.  offsets: a CUDA int64 tensor of at least n + 1 entries (n
+        defaults to its length - 1), or a raw device pointer with `n` given.  `stream`: a torch.cuda.Stream or a raw cudaStream_t.
+        src_bytes = offsets[n] - offsets[0].  Given, it is taken as it is and the call only enqueues (it may be captured in a CUDA
+        graph).  When None it is read from the device: the device is synchronised and offsets[0] and offsets[n] are copied back,
+        so that form is neither asynchronous nor capturable.  The source must stay untouched until the work on `stream` has run."""
+        if isinstance(offsets, int):
+            if n is None:
+                raise ValueError("offsets given as a raw pointer: pass n")
+        else:
+            import torch
+
+            if offsets.dtype != torch.int64:
+                raise ValueError(f"offsets must be an int64 tensor, not {offsets.dtype}")
+            if n is None:
+                n = offsets.numel() - 1
+            if offsets.numel() < n + 1:
+                raise ValueError(f"offsets holds {offsets.numel()} entries; {n} units need {n + 1}")
+        if not isinstance(src, int):
+            import torch
+
+            if src.dtype != torch.uint8:
+                raise ValueError(f"src must be a uint8 tensor, not {src.dtype}")
+        po, ps = _dev_ptr(offsets), _dev_ptr(src)
+        if src_bytes is None and n > 0:
+            import torch
+
+            torch.cuda.synchronize()
+            ends = np.zeros(2, dtype=np.uint64)
+            with self.ctx.lock:
+                self.ctx.check(self.ctx.lib.cf_copy_to_host(self.ctx.h, ends.ctypes.data, po, 8), "cf_copy_to_host")
+                self.ctx.check(self.ctx.lib.cf_copy_to_host(self.ctx.h, ends.ctypes.data + 8, po + 8 * n, 8), "cf_copy_to_host")
+            src_bytes = int(ends[1]) - int(ends[0])
+            if not isinstance(src, int) and src.numel() < int(ends[1]):
+                raise ValueError(f"src holds {src.numel()} bytes; offsets[{n}] = {int(ends[1])}")
+        elif src_bytes is not None and not isinstance(src, int) and src.numel() < src_bytes:
+            raise ValueError(f"src holds {src.numel()} bytes; src_bytes = {src_bytes}")
+        st = getattr(stream, "cuda_stream", stream)
+        with self.ctx.lock:
+            self.ctx.check(self.ctx.lib.cf_batch_pack_device(self.ctx.h, self.h, ps, po, n, src_bytes or 0, st or None), "cf_batch_pack_device")
+
     def __del__(self):
         try:
             self.ctx.lib.cf_batch_free(self.h)
@@ -333,6 +378,9 @@ class Run:
         batch.upload(stream, offsets, cuda_stream=s)              # on the same stream
         run.enqueue(prog, batch, STAGES, None, 0, verdicts, out_offsets, out, bitmaps_full, stream=s)
         needed = run.finish()                                     # 0, or the capacity `out` needs; CfError on failure
+
+    After a finish that returned 0, `gathered_bytes` is the byte count of the texts in `out` (out_offsets[n]): what
+    Batch.pack_device needs to feed them to another run on the device, e.g. to TOON-encode the units flagged CF_V_RESUBMIT.
     """
 
     def __init__(self, ctx: Context, max_units: int, max_bytes: int, sub_arena_bytes: int = 1 << 20):
@@ -341,6 +389,7 @@ class Run:
         with ctx.lock:
             ctx.check(ctx.lib.cf_run_create(ctx.h, max_units, max_bytes, sub_arena_bytes, byref(self.h)), "cf_run_create")
         self._keep = ()
+        self.gathered_bytes: Optional[int] = None   # out_offsets[n] of the last finish() that gathered every text into `out`
 
     def enqueue(self, prog: Optional[Program], batch: Batch, stage_mask: int, d_unit_stages, toon_flags: int, verdicts, out_offsets, out,
                 bitmaps_full=None, stream=0, mask_max_depth: int = 10) -> None:
@@ -384,11 +433,13 @@ class Run:
         `out` must hold when it was too small (CF_E_CAPACITY: verdicts and out_offsets are valid, `out` is untouched); raises
         CfError on any other failure."""
         need = c_uint64(0)
+        self.gathered_bytes = None
         with self.ctx.lock:
             rc = self.ctx.lib.cf_run_finish(self.ctx.h, self.h, byref(need))
         if rc == N.CF_E_CAPACITY and need.value:
             return int(need.value)
         self.ctx.check(rc, "cf_run_finish")
+        self.gathered_bytes = int(need.value)
         return 0
 
     def __del__(self):
