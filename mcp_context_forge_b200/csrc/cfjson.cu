@@ -379,7 +379,7 @@ int cf_toon(cf_ctx* ctx, cf_batch* b, uint32_t flags, uint8_t* d_out, uint32_t* 
 }
 
 #ifdef CF_TOON_PHASES
-// Phase-timing builds only (json_tp.h TP_PHASE): out[k] = the cycles all warps spent in phase k since the last call, which clears them.
+// Phase-timing builds only (json_tp.h TP_PHASE): out[k], k < PH_N, = the cycles all warps spent in phase k since the last call, which clears them.
 int cf_toon_phase_cycles(unsigned long long* out) {
   const size_t n = (size_t)cftp::PH_WARPS * (cftp::PH_N + 1);
   unsigned long long* h = (unsigned long long*)calloc(n, sizeof(unsigned long long));

@@ -43,7 +43,11 @@ enum : uint32_t { FB_NUM_EXACT = 1, FB_KEY_ESCAPE = 2, FB_TOK_CAP = 3, FB_KH_CAP
 // ---- phase timing: build option CF_TOON_PHASES, off in the shipped library (tools/toon_phase_breakdown.py builds it) ----
 // Lane 0 of each warp adds the clock64() cycles of each phase to the warp's row of toon_phase_cycles (warp slots wrap around at
 // PH_WARPS).  Column PH_N is the warp's "inside the resolve retry" flag: the retry's cycles count once, in PH_RESOLVE.
-enum : uint32_t { PH_TOKENIZE = 0, PH_AN_GENERIC = 1, PH_AN_TABLE = 2, PH_EM_GENERIC = 3, PH_EM_TABLE = 4, PH_RESOLVE = 5, PH_N = 6 };
+// The PH_TK_* columns split PH_TOKENIZE: the step's loads and window shift, the mask algebra and warp scans, the per-kind ring
+// passes, the classification batches (tok_batch, the long-string checks included) and, inside them, the whole-warp long-string
+// checks alone.
+enum : uint32_t { PH_TOKENIZE = 0, PH_AN_GENERIC = 1, PH_AN_TABLE = 2, PH_EM_GENERIC = 3, PH_EM_TABLE = 4, PH_RESOLVE = 5,
+                  PH_TK_LOAD = 6, PH_TK_MASKS = 7, PH_TK_RING = 8, PH_TK_BATCH = 9, PH_TK_LONG = 10, PH_N = 11 };
 #if defined(CF_TOON_PHASES) && defined(__CUDACC__)
 static const uint32_t PH_WARPS = 1u << 16;
 __device__ unsigned long long toon_phase_cycles[PH_WARPS * (PH_N + 1)];
@@ -54,9 +58,14 @@ TP_FN void ph_add(uint32_t k, unsigned long long t0) {
 }
 TP_FN void ph_in_retry(bool on) { if (tpw::lane() == 0) ph_row()[PH_N] = on ? 1ull : 0ull; }
 #define TP_PHASE(k, ...) do { const unsigned long long ph_t0_ = clock64(); __VA_ARGS__; ph_add((k), ph_t0_); } while (0)
+// a sub-phase whose code may `break` out of the enclosing loop: TP_MARK(t) starts it, TP_LAP(k, t) adds its cycles and restarts t
+#define TP_MARK(t) unsigned long long t = clock64()
+#define TP_LAP(k, t) do { ph_add((k), (t)); (t) = clock64(); } while (0)
 #else
 TP_FN void ph_in_retry(bool) {}
 #define TP_PHASE(k, ...) do { __VA_ARGS__; } while (0)
+#define TP_MARK(t) do {} while (0)
+#define TP_LAP(k, t) do {} while (0)
 #endif
 
 // ---- tokens --------------------------------------------------------------------------------------------------------
@@ -90,7 +99,8 @@ static const uint32_t TOK_WIN = 192;      // tokens of one 1 KiB step pushed thr
 static const uint32_t UNSET = 0xFFFFFFFFu;
 struct Shared {
   unsigned long long sbar_bar;         // mbarrier of the staging buffer's bulk TMA loads (initialised by the kernel)
-  uint32_t sbar_phase, sbar_pad;
+  uint32_t sbar_phase;
+  uint32_t utf8_bad;                   // tokenize: unit position of the first byte where its UTF-8 fails (UNSET: none so far)
   // analyze: container stack            | emit: frame stack (same storage)
   uint32_t open_idx[MAXD];             // token index of the opener      | frame mode
   uint32_t cnt[MAXD];                  // children (values) so far       | children so far
@@ -429,27 +439,6 @@ TP_SLOW bool string_slow(const uint8_t* s, uint32_t n, uint32_t pos, uint32_t le
   return cfj::parse_string(s, n, &p, sf, &h) && p == pos + len + 1;
 }
 
-// Strict UTF-8 over s[a .. a+len), the whole warp on one (long) string, lane i <-> byte i of a 32-byte chunk: a byte must be a
-// continuation byte exactly when one of the three bytes before it is a lead that reaches it, leads are C2..F4, and the second
-// byte of E0 / ED / F0 / F4 sequences is range-checked (no overlongs, no surrogates, nothing above U+10FFFF) — what
-// cfj::parse_string checks one code point at a time.  The byte behind the string is its closing quote: a truncated tail fails.
-TP_SLOW bool warp_utf8_valid(const uint8_t* s, uint32_t a, uint32_t len) {
-  const uint32_t l = tpw::lane();
-  bool bad = false;
-  for (uint32_t base = 0; base <= len; base += 32) {
-    const uint32_t i = base + l;
-    if (i <= len) {
-      const uint32_t p = a + i;
-      const uint32_t b0 = s[p], b1 = i >= 1 ? s[p - 1] : 0u, b2 = i >= 2 ? s[p - 2] : 0u, b3 = i >= 3 ? s[p - 3] : 0u;
-      const bool cont = (b0 & 0xC0u) == 0x80u;
-      const bool must = b1 >= 0xC0u || b2 >= 0xE0u || b3 >= 0xF0u;
-      if (cont != must) bad = true;
-      if (b0 >= 0x80u && !cont && (b0 < 0xC2u || b0 > 0xF4u)) bad = true;
-      if (cont && ((b1 == 0xE0u && b0 < 0xA0u) || (b1 == 0xEDu && b0 > 0x9Fu) || (b1 == 0xF0u && b0 < 0x90u) || (b1 == 0xF4u && b0 > 0x8Fu))) bad = true;
-    }
-  }
-  return !tpw::any(bad);
-}
 TP_FN uint32_t utf8_first_cp(const uint8_t* b) {
   const uint32_t c = b[0];
   if (c < 0x80) return c;
@@ -458,7 +447,7 @@ TP_FN uint32_t utf8_first_cp(const uint8_t* b) {
   for (uint32_t k = 1; k <= need; ++k) cp = (cp << 6) | (b[k] & 0x3Fu);
   return cp;
 }
-static const uint32_t LONG_HI = 96;      // non-ASCII / escaped strings at least this long are validated by the whole warp
+static const uint32_t LONG_HI = 96;      // non-ASCII / escaped strings at least this long: escapes checked by the whole warp, UTF-8 by utf8_bad
 
 // Escapes of a long string s[a .. a+len), whole warp: every unescaped backslash must start one of JSON's two-character escapes
 // (a \uXXXX escape makes the caller take the sequential validator: its code point decides the predicates).
@@ -504,6 +493,64 @@ TP_FN const uint8_t* in_window(const uint8_t* s, const uint8_t* win, uint32_t wl
   const uint32_t d = pos - wlo;                       // wraps to a huge value when pos < wlo
   return (d < WIN && len <= WIN - d) ? win + d : s + pos;
 }
+// Strict UTF-8 over the step's bytes in the window (stage[1024, 2048)), lane l on its 32 bytes and the three in front of them (the
+// previous step's last ones for lane 0: stage[1021, 1024)); bytes outside [lead, vend) count as blanks.  A byte must be a
+// continuation byte exactly when one of the three bytes before it is a lead that reaches it, leads are C2..F4, and the second byte
+// of E0 / ED / F0 / F4 sequences is range-checked (no overlongs, no surrogates, nothing above U+10FFFF): what cfj::parse_string
+// checks one code point at a time.  The first failing position of the unit goes to sh.utf8_bad; tok_batch raises it at the
+// string that holds it, so the unit's status is the one a string-by-string check gives.  (Outside strings, a non-ASCII byte
+// fails its scalar run anyway.)
+// SWAR, four bytes per step of the lane's walk: 0x80 in every byte of x (bytes b0) that breaks a rule, pw = the word in front.
+TP_FN uint32_t utf8_bad_bytes(uint32_t x, uint32_t pw) {
+  const uint32_t p1 = (x << 8) | (pw >> 24), p2 = (x << 16) | (pw >> 16), p3 = (x << 24) | (pw >> 8);   // b1, b2, b3 of each byte
+  const uint32_t cont = swar_eq(x & 0xC0C0C0C0u, 0x80u);
+  const uint32_t must = swar_eq(p1 & 0xC0C0C0C0u, 0xC0u) | swar_eq(p2 & 0xE0E0E0E0u, 0xE0u) | swar_eq(p3 & 0xF0F0F0F0u, 0xF0u);
+  // leads C0, C1 and F5..FF (F5 and up: the low seven bits plus 0x0B carry into bit 7)
+  const uint32_t bad_lead = x & ~cont & (swar_eq(x & 0xFEFEFEFEu, 0xC0u) | (x & ((x & 0x7F7F7F7Fu) + 0x0B0B0B0Bu)));
+  // second bytes: after E0 at least A0 (bit 5), after ED at most 9F, after F0 at least 90 (bit 4 or 5), after F4 at most 8F
+  const uint32_t b5 = x << 2, b45 = (x << 2) | (x << 3);
+  const uint32_t second = cont & ((swar_eq(p1, 0xE0u) & ~b5) | (swar_eq(p1, 0xEDu) & b5) | (swar_eq(p1, 0xF0u) & ~b45) | (swar_eq(p1, 0xF4u) & b45));
+  return ((cont ^ must) | bad_lead | second) & 0x80808080u;
+}
+// the bytes of x (at virtual offsets [pos, pos + 4)) outside [lo, hi) -> blanks
+TP_SLOW uint32_t utf8_blank(uint32_t x, int64_t pos, uint32_t lo, uint32_t hi) {
+  for (uint32_t j = 0; j < 4; ++j)
+    if (pos + j < (int64_t)lo || pos + j >= (int64_t)hi) x = (x & ~(0xFFu << (8 * j))) | (0x20u << (8 * j));
+  return x;
+}
+TP_FN void step_utf8_walk(const uint8_t* stage, Shared& sh, uint32_t v, uint32_t lead, uint32_t vend, bool mine) {
+  const uint32_t l = tpw::lane();
+  uint32_t first = UNSET;
+  if (mine) {
+    const uint32_t* p = reinterpret_cast<const uint32_t*>(stage + 1024 + 32 * l);
+    const bool edge = v < lead + 4 || v + 32 > vend;         // some byte of the lane or of the word in front is not the unit's
+    uint32_t pw = p[-1];                                     // lane 0: the previous step's last word
+    if (edge) pw = utf8_blank(pw, (int64_t)v - 4, lead, vend);
+#pragma unroll 1
+    for (uint32_t k = 0; k < 8; ++k) {
+      uint32_t x = p[k];
+      if (edge) x = utf8_blank(x, (int64_t)v + 4 * k, lead, vend);
+      const uint32_t bad = utf8_bad_bytes(x, pw);
+      if (bad) { first = v + 4 * k + ((tpw::ffs(bad) - 1) >> 3) - lead; break; }
+      pw = x;
+    }
+  }
+  for (uint32_t d = 16; d; d >>= 1) { const uint32_t o = tpw::shfl(first, (l + d) & 31u); first = o < first ? o : first; }
+  if (l == 0 && sh.utf8_bad == UNSET) sh.utf8_bad = first;
+  tpw::sync();
+}
+// ASCII steps (the common case) pay two shared loads, a shuffle and a vote; only steps with a non-ASCII byte walk their bytes.
+// (Out of line, the walk measured slower on every payload shape: the call spills the tokenizer's carries around it.)
+TP_FN void step_utf8(const uint8_t* stage, Shared& sh, uint32_t v, uint32_t lead, uint32_t vend) {
+  const uint32_t l = tpw::lane();
+  const uint4 a = *reinterpret_cast<const uint4*>(stage + 1024 + 32 * l), b = *reinterpret_cast<const uint4*>(stage + 1024 + 32 * l + 16);
+  const uint32_t hi = (a.x | a.y | a.z | a.w | b.x | b.y | b.z | b.w) & 0x80808080u;
+  uint32_t tail = tpw::shfl_up(b.w, 1);               // the three bytes in front of the lane (their lead bytes may reach into it)
+  if (l == 0) tail = *reinterpret_cast<const uint32_t*>(stage + 1020);
+  const bool mine = hi != 0 || (tail & 0x80808000u) != 0;
+  if (tpw::any(mine)) step_utf8_walk(stage, sh, v, lead, vend, mine);
+}
+
 TP_FN void tok_batch(const uint8_t* s, uint32_t n, GTok* toks, uint32_t tok_cap, Shared& sh, TokState& st, uint32_t head, uint32_t m, uint32_t la_ncolon,
                      const uint8_t* win, uint32_t wlo) {
   const uint32_t l = tpw::lane();
@@ -559,12 +606,15 @@ TP_FN void tok_batch(const uint8_t* s, uint32_t n, GTok* toks, uint32_t tok_cap,
     }
     if (isK) kind = K_KEY;
   }
-  // long non-ASCII strings without escapes: strict UTF-8 by the whole warp, one string after the other; what is left of the
-  // predicates needs the first and the last code point only (no escapes: the text is the bytes; no digit in front: not number-like)
+  // long non-ASCII or escaped strings, one after the other: UTF-8 was checked step by step (Shared::utf8_bad, the first failing
+  // position of the unit: a string that holds it, closing quote included, is not JSON; a failure in front of it stopped an earlier
+  // batch), escapes by the whole warp; what is left of the predicates needs the first and the last code point only (no digit in
+  // front: not number-like)
+  TP_MARK(t_long);
   for (uint32_t lm = tpw::ballot(long_hi); lm; lm &= lm - 1) {
     const uint32_t j = tpw::ffs(lm) - 1;
     const uint32_t jpos = tpw::shfl(pos, j), jlen = tpw::shfl(len, j), jmeta = tpw::shfl(meta, j);
-    const bool ok = !(jmeta & RM_HI) || warp_utf8_valid(s, jpos, jlen);
+    const bool ok = !(jmeta & RM_HI) || sh.utf8_bad - jpos > jlen;
     const uint32_t xe = (jmeta & RM_BS) ? warp_escapes(s, jpos, jlen) : 0u;
     if (l == j) {
       if (!ok || (xe & XE_BAD)) bad = true;
@@ -602,6 +652,7 @@ TP_FN void tok_batch(const uint8_t* s, uint32_t n, GTok* toks, uint32_t tok_cap,
       }
     }
   }
+  TP_LAP(PH_TK_LONG, t_long);
   if (len > GT_MAXLEN) { if (kind == K_NUM || kind == K_LIT) unsup = true; else if (!fb) fb = FB_TOO_LONG; len = 0; }
   if (st.ntok + m > tok_cap) fb = FB_TOK_CAP;
   else if (act) { GTok t; t.pos = pos; t.w = gt_make(kind, fl, ncomma, ncolon, kind <= K_CLOSE_ARR ? 0u : len); toks[st.ntok + l] = t; }
@@ -631,26 +682,25 @@ TP_FN int tokenize(const uint8_t* s, uint32_t n, GTok* toks, uint32_t tok_cap, S
   uint32_t c_bits = 0, c_sep = 0 /* commas | colons << 16 since the last token */;
   uint32_t c_open = 0;                                // string open across steps: position of its opening quote
   uint32_t head = 0, rcount = 0;
+  if (l == 0) sh.utf8_bad = UNSET;
+  tpw::sync();
   for (uint32_t vb = 0; vb < vend; vb += 1024) {
+    TP_MARK(t_tk);
     const uint32_t v = vb + 32 * l;                   // virtual offset of this lane's first byte
-    uint32_t w[8];
-    if (v < vend) {
-      const uint4 a = *reinterpret_cast<const uint4*>(s0 + v), b = *reinterpret_cast<const uint4*>(s0 + v + 16);
-      w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w; w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
-    } else {
-#pragma unroll
-      for (uint32_t k = 0; k < 8; ++k) w[k] = 0x20202020u;
-    }
     // source window for the classification batches: [previous step | this step]
     {
+      uint4 c0;                                       // lanes past the end: blanks
+      c0.x = c0.y = c0.z = c0.w = 0x20202020u;
+      uint4 c1 = c0;
+      if (v < vend) { c0 = *reinterpret_cast<const uint4*>(s0 + v); c1 = *reinterpret_cast<const uint4*>(s0 + v + 16); }
       const uint4 p0 = *reinterpret_cast<const uint4*>(stage + 1024 + 32 * l), p1 = *reinterpret_cast<const uint4*>(stage + 1024 + 32 * l + 16);
       tpw::sync();
       *reinterpret_cast<uint4*>(stage + 32 * l) = p0; *reinterpret_cast<uint4*>(stage + 32 * l + 16) = p1;
-      uint4 c0, c1;
-      c0.x = w[0]; c0.y = w[1]; c0.z = w[2]; c0.w = w[3]; c1.x = w[4]; c1.y = w[5]; c1.z = w[6]; c1.w = w[7];
       *reinterpret_cast<uint4*>(stage + 1024 + 32 * l) = c0; *reinterpret_cast<uint4*>(stage + 1024 + 32 * l + 16) = c1;
       tpw::sync();
     }
+    step_utf8(stage, sh, v, lead, vend);
+    TP_LAP(PH_TK_LOAD, t_tk);
     const uint32_t wlo = vb - 1024 - lead;             // unit position of stage[0] (wraps for the first step: nothing lies there)
     // The step's masks are rebuilt for every window of TOK_WIN tokens, from its bytes in the staging buffer and the carries at the
     // step's start, so that none of them is live across the classification batches (tok_batch): 80 registers hold either, not both.
@@ -658,6 +708,7 @@ TP_FN int tokenize(const uint8_t* s, uint32_t n, GTok* toks, uint32_t tok_cap, S
     const uint32_t c_bits0 = c_bits, c_sep0 = c_sep, c_open0 = c_open;
     for (uint32_t done = 0;; done += TOK_WIN) {
       c_bits = c_bits0; c_sep = c_sep0; c_open = c_open0;
+      uint32_t w[8];
       {
         const uint4 a = *reinterpret_cast<const uint4*>(stage + 1024 + 32 * l), b = *reinterpret_cast<const uint4*>(stage + 1024 + 32 * l + 16);
         w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w; w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
@@ -764,6 +815,7 @@ TP_FN int tokenize(const uint8_t* s, uint32_t n, GTok* toks, uint32_t tok_cap, S
       const uint32_t lane_off = incl - cntT, total = tpw::shfl(incl, 31);
       uint32_t other_nx = tpw::shfl_down(other, 1);       // the next lane's scalar bytes: a run may continue there
       if (l == 31) other_nx = 0xFFFFFFFFu;                // unknown: treated as "continues" -> RM_OPENEND
+      TP_LAP(PH_TK_MASKS, t_tk);
       if (done >= total) break;                          // no (more) tokens in this step
       {
         const uint32_t win = total - done > TOK_WIN ? TOK_WIN : total - done;
@@ -809,12 +861,14 @@ TP_FN int tokenize(const uint8_t* s, uint32_t n, GTok* toks, uint32_t tok_cap, S
   #undef TP_TOKEN_EPILOGUE
         rcount += win;
         tpw::sync();
+        TP_LAP(PH_TK_RING, t_tk);
         while (rcount >= 33 && !st.status) {
           const uint32_t la = (rmeta[(head + 32) & (RING - 1)] >> RM_NCOLON_SH) & 3u;
           tok_batch(s, n, toks, tok_cap, sh, st, head, 32, la, stage, wlo);
           head += 32; rcount -= 32;
         }
         tpw::sync();
+        TP_LAP(PH_TK_BATCH, t_tk);
       }
       if (st.status || done + TOK_WIN >= total) break;
     }
@@ -827,7 +881,7 @@ TP_FN int tokenize(const uint8_t* s, uint32_t n, GTok* toks, uint32_t tok_cap, S
     while (rcount && !st.status) {
       const uint32_t m = rcount > 32 ? 32u : rcount;
       const uint32_t la = rcount > 32 ? ((rmeta[(head + 32) & (RING - 1)] >> RM_NCOLON_SH) & 3u) : 0u;
-      tok_batch(s, n, toks, tok_cap, sh, st, head, m, la, stage, wlo);
+      TP_PHASE(PH_TK_BATCH, tok_batch(s, n, toks, tok_cap, sh, st, head, m, la, stage, wlo));
       head += m; rcount -= m;
     }
   }

@@ -7,6 +7,12 @@ each) and prints, per case, the clock64() cycles per unit each phase took (summe
   an_generic    analyze's generic bracket walk (an_batch)       an_table   analyze's table rows (an_rows)
   em_generic    emit's generic walk (em_batch)                  em_table   emit's table rows (em_rows)
   resolve       the in-place retry of mixed list-item arrays (its analyze and emit count here only)
+and, on a second line per case, tokenize split into its parts (cycles per unit and share of tokenize):
+  load          the step's loads and the source window's shift
+  masks         mask algebra and the warp scans (separators, open strings, token ranks)
+  ring          the per-kind ring passes (brackets, strings, scalar runs)
+  classify      tok_batch without the long-string checks
+  long          tok_batch's per-string pass over long non-ASCII / escaped strings (warp_escapes, first / last code point)
 The timing itself costs cycles (clock reads, one atomic per phase call), so the numbers are for comparing phases and builds, not
 for adding up to the stage time.
 
@@ -28,6 +34,8 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 PHASES = ("tokenize", "an_generic", "an_table", "em_generic", "em_table", "resolve")   # json_tp.h PH_*
+TK_PHASES = ("load", "masks", "ring", "batch", "long")                                # json_tp.h PH_TK_* (batch includes long)
+TK_SHOWN = ("load", "masks", "ring", "classify", "long")
 
 
 def build_variant(outdir: str) -> str:
@@ -73,7 +81,7 @@ def main():
     read = ctypes.CDLL(so).cf_toon_phase_cycles
     read.restype = ctypes.c_int
     read.argtypes = [ctypes.POINTER(ctypes.c_ulonglong)]
-    cyc = (ctypes.c_ulonglong * len(PHASES))()
+    cyc = (ctypes.c_ulonglong * (len(PHASES) + len(TK_PHASES)))()
 
     payloads = bench.make_payloads()
     by_shape = {}
@@ -103,10 +111,15 @@ def main():
         torch.cuda.synchronize()
         assert read(cyc) == 0
         per = {p: cyc[k] / (args.reps * n) for k, p in enumerate(PHASES)}
+        tk = {p: cyc[len(PHASES) + k] / (args.reps * n) for k, p in enumerate(TK_PHASES)}
+        tk["classify"] = tk.pop("batch") - tk["long"]
         tot = sum(per.values())
-        out["cases"][name] = {"cycles_per_unit": per, "share": {p: (v / tot if tot else 0.0) for p, v in per.items()}}
+        ttk = per["tokenize"]
+        out["cases"][name] = {"cycles_per_unit": per, "share": {p: (v / tot if tot else 0.0) for p, v in per.items()},
+                              "tokenize_cycles_per_unit": tk, "tokenize_share": {p: (v / ttk if ttk else 0.0) for p, v in tk.items()}}
         print(f"{name:5s}" + "".join(f"{per[p]:12.0f}" for p in PHASES) + f"{tot:12.0f}")
-        print(f"{'':5s}" + "".join(f"{100 * per[p] / tot if tot else 0:11.1f}%" for p in PHASES), flush=True)
+        print(f"{'':5s}" + "".join(f"{100 * per[p] / tot if tot else 0:11.1f}%" for p in PHASES))
+        print(f"{'':5s}  tokenize:" + "".join(f"  {p} {tk[p]:.0f} ({100 * tk[p] / ttk if ttk else 0:.1f}%)" for p in TK_SHOWN), flush=True)
     if args.json:
         with open(args.json, "w") as f:
             json.dump(out, f, indent=1)
