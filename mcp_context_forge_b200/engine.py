@@ -157,9 +157,17 @@ class PinnedBuffer:
     def __init__(self, ctx: Context, nbytes: int):
         self.ctx = ctx
         self.p = c_void_p()
+        self.nbytes = nbytes
         with ctx.lock:
             ctx.check(ctx.lib.cf_host_alloc(ctx.h, nbytes, byref(self.p)), "cf_host_alloc")
-        self.array = np.ctypeslib.as_array(ctypes.cast(self.p, ctypes.POINTER(ctypes.c_uint8)), shape=(nbytes,))
+
+    @property
+    def array(self) -> np.ndarray:
+        """A view of the buffer that keeps the buffer alive: texts sliced from it stay readable after the Batch that held it is gone
+        or has grown a bigger one."""
+        view = (ctypes.c_uint8 * self.nbytes).from_address(self.p.value)
+        view.owner = self
+        return np.frombuffer(view, dtype=np.uint8)
 
     def __del__(self):
         try:
@@ -329,7 +337,7 @@ def run_batch(prog: Optional[Program], batch: Batch, stream, offsets: np.ndarray
     # the output buffer lives with the Batch, is page-locked and only grows.  NOTE: the returned `out` is a view of it — it is
     # overwritten by the next run_batch on this Batch (callers slice/copy what they keep).
     pin = getattr(batch, "_out_pin", None)
-    cap = max(nbytes, 1 << 12) if pin is None else len(pin.array)
+    cap = max(nbytes, 1 << 12) if pin is None else pin.nbytes
     if pin is None:
         pin = batch._out_pin = PinnedBuffer(ctx, cap)
     out = pin.array

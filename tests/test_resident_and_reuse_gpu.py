@@ -3,8 +3,10 @@ left in HBM), one long-lived Batch that takes uploads of very different sizes on
 batchers do), and the host-side cache of a batch's unit lengths in cf_sub_host across a freed and re-allocated batch.
 Everything is checked against the oracles and against the host-buffer entry points on a fresh batch."""
 import ctypes
+import gc
 import json
 import re
+import weakref
 
 import numpy as np
 import pytest
@@ -356,3 +358,23 @@ def test_sub_sizing_follows_a_new_batch_at_a_freed_batch_address():
     b2.upload(s, o)
     assert [x.decode() for x in engine.sub_host(p, b2, [0, 1])] == [ref.regex_apply_str(rules, u) for u in second]
     del bb
+
+
+def test_run_batch_texts_outlive_their_batch():
+    """The texts run_batch returns are a view of the Batch's page-locked output buffer.  The view keeps that buffer alive: the texts
+    of a Batch that was dropped right after the call (a temporary argument) read back whole, and the buffer is freed with the last view."""
+    ctx = engine.Context.get()
+    texts = [synth.payload("A", 2048, seed=s) for s in range(16)] + [synth.payload("B", 2048, seed=s) for s in range(4)]
+    stream, offs = engine.pack_units(texts)
+    batch = engine.Batch(ctx, len(stream), len(texts))
+    v, out, oo, _ = engine.run_batch(None, batch, stream, offs, N.CF_STAGE_TOON)
+    pin = weakref.ref(batch._out_pin)
+    del batch
+    gc.collect()
+    assert pin() is not None
+    got = [out[int(oo[i]):int(oo[i + 1])].tobytes().decode() if v["aux"][i] == engine.TOON_CONVERTED else None for i in range(len(texts))]
+    assert got == [toon_ref.process_text(t, 0, 1 << 30) for t in texts]
+    assert any(got)
+    del out
+    gc.collect()
+    assert pin() is None

@@ -3,8 +3,9 @@ the REFERENCE'S OWN plugin classes (kind: plugins.regex_filter.search_replace.Se
 and `BatchedPluginManager` loading this repo's drop-ins (kind: mcp_context_forge_b200.plugins....) on the engine's CPU simulator — same priorities,
 modes, conditions and hook policies, random waves of concurrent requests on the three hooks of the path, violations as results and as
 exceptions.  Every request's (continue_processing, modified payload, violation, metadata) or raised error must be equal.
-With --record the reference itself is run and its answers are stored (tools/ref_answers.py); without it they are read back from tests/golden/.
-usage: python tools/fuzz_chain_vs_reference.py [seed] [rounds] [requests per wave] [--record]"""
+With --record the reference itself is run and its answers are stored (tools/ref_answers.py); without it they are read back from tests/golden/
+(fuzz_chain.json.gz, or NAME.json.gz with --answers NAME).  --device runs the batched manager's launches on the GPU instead of the simulator.
+usage: python tools/fuzz_chain_vs_reference.py [seed] [rounds] [requests per wave] [--record | --device] [--answers NAME]"""
 import asyncio
 import json
 import os
@@ -18,7 +19,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 import gen_golden  # noqa: E402
-from ref_answers import Answers, canon  # noqa: E402
+from ref_answers import Answers, canon, split_argv  # noqa: E402
 
 OURS = {"harm": "mcp_context_forge_b200.plugins.harmful_content_detector.HarmfulContentDetectorPlugin", "deny": "mcp_context_forge_b200.plugins.deny_filter.DenyListPlugin",
         "regex": "mcp_context_forge_b200.plugins.regex_filter.SearchReplacePlugin", "sql": "mcp_context_forge_b200.plugins.sql_sanitizer.SQLSanitizerPlugin",
@@ -70,13 +71,12 @@ def render(plugs, kinds, fail_all=False):
 
 
 def main() -> int:
-    record = "--record" in sys.argv
-    argv = [a for a in sys.argv[1:] if a != "--record"]
+    argv, record, device, name = split_argv(sys.argv[1:])
     seed = int(argv[0]) if len(argv) > 0 else 1
     rounds = int(argv[1]) if len(argv) > 1 else 20
     nreq = int(argv[2]) if len(argv) > 2 else 60
-    answers = Answers("chain", [seed, rounds, nreq], record)
-    gen_golden.install_shims()
+    answers = Answers("chain", [seed, rounds, nreq], record, name)
+    gen_golden.install_shims(reference=record)
     import logging
 
     import pytest
@@ -88,7 +88,8 @@ def main() -> int:
     from mcp_context_forge_b200.regex_frontend import UnsupportedPattern
 
     logging.disable(logging.ERROR)
-    hostsim_batcher.install(pytest.MonkeyPatch())
+    if not device:
+        hostsim_batcher.install(pytest.MonkeyPatch())
     rng = random.Random(seed)
     loop = asyncio.new_event_loop()
     t0 = time.time()
@@ -146,7 +147,7 @@ def main() -> int:
                                       "\n  product  ", repr(tm.norm(v))[:600])
             slow += bat.slow_path_calls
     answers.finish()
-    print(f"seed={seed} chains={rounds} rejected_loudly={rejected} requests={n} slow_path_calls={slow} bad={bad} time={time.time() - t0:.1f}s")
+    print(f"seed={seed} chains={rounds} rejected_loudly={rejected} requests={n} compared={n} slow_path_calls={slow} bad={bad} time={time.time() - t0:.1f}s")
     return 1 if bad else 0
 
 

@@ -1,8 +1,9 @@
 """Differential fuzz of the json_repair drop-in (on the engine's CPU simulator: JSON kernel source for "does it parse",
 substitution routines for the trailing-comma rule) against the REFERENCE'S OWN plugins/json_repair/json_repair.py, imported unmodified from
 /root/reference (orjson stood in for by the strict stdlib parser; texts that would expose an orjson / json delta are skipped).
-With --record the reference itself is run and its answers are stored (tools/ref_answers.py); without it they are read back from tests/golden/.
-usage: python tools/fuzz_json_repair_vs_reference.py [seed] [cases] [--record]"""
+With --record the reference itself is run and its answers are stored (tools/ref_answers.py); without it they are read back from tests/golden/
+(fuzz_json_repair.json.gz, or NAME.json.gz with --answers NAME).  --device runs the drop-in's launches on the GPU instead of the simulator.
+usage: python tools/fuzz_json_repair_vs_reference.py [seed] [cases] [--record | --device] [--answers NAME]"""
 import os
 import random
 import re
@@ -15,18 +16,17 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 import gen_golden  # noqa: E402
 from fuzz_toon_tp import make_gen  # noqa: E402
-from ref_answers import Answers  # noqa: E402
+from ref_answers import Answers, split_argv  # noqa: E402
 
 _DELTA = re.compile(r"\d{18,}|[eE][+-]?\d{3,}|\\u[dD][89a-fA-F]|NaN|Infinity")
 
 
 def main() -> int:
-    record = "--record" in sys.argv
-    argv = [a for a in sys.argv[1:] if a != "--record"]
+    argv, record, device, name = split_argv(sys.argv[1:])
     seed = int(argv[0]) if len(argv) > 0 else 1
     n = int(argv[1]) if len(argv) > 1 else 3000
-    answers = Answers("json_repair", [seed, n], record)
-    gen_golden.install_shims()
+    answers = Answers("json_repair", [seed, n], record, name)
+    gen_golden.install_shims(reference=record)
     import pytest
     from cpex.framework import GlobalContext, PluginConfig, PluginContext, ToolPostInvokePayload
 
@@ -34,7 +34,8 @@ def main() -> int:
     import test_json_repair as tj
     from mcp_context_forge_b200.plugins.json_repair import JSONRepairPlugin
 
-    hostsim_batcher.install(pytest.MonkeyPatch())
+    if not device:
+        hostsim_batcher.install(pytest.MonkeyPatch())
     if record:
         from plugins.json_repair.json_repair import JSONRepairPlugin as RefPlugin
 
@@ -70,7 +71,7 @@ def main() -> int:
         print("BAD", str(exc)[:1500])
         return 1
     answers.finish()
-    print(f"seed={seed} cases={len(cases)} repaired={sum(c['modified'] for c in cases)} bad=0 time={time.time() - t0:.1f}s")
+    print(f"seed={seed} cases={len(cases)} compared={len(cases)} repaired={sum(c['modified'] for c in cases)} bad=0 time={time.time() - t0:.1f}s")
     return 0
 
 

@@ -2,8 +2,11 @@
 serialisation) against the REFERENCE'S OWN Python twin of the Rust crate (`mcpgateway/middleware/request_logging_middleware.py:83-291`, its pure
 functions exec'd unmodified from /root/reference as tools/gen_golden.py does) — generated key names (token vocabulary x separators x casings),
 random nested bodies, max_depth 0..12 — and against the oracle (oracle/mask_ref.py) byte for byte.
-With --record the reference itself is run and its answers are stored (tools/ref_answers.py); without it they are read back from tests/golden/.
-usage: python tools/fuzz_mask_vs_reference.py [seed] [keys] [bodies] [--record]"""
+With --record the reference itself is run and its answers are stored (tools/ref_answers.py); without it they are read back from tests/golden/
+(fuzz_mask.json.gz, or NAME.json.gz with --answers NAME).
+--device runs the same comparisons on the GPU: every key through one classify_keys_kernel launch, the bodies through cf_mask_host and through
+cf_run_batch(CF_STAGE_MASK), one launch of each per max_depth, and the module's launches for real.
+usage: python tools/fuzz_mask_vs_reference.py [seed] [keys] [bodies] [--record | --device] [--answers NAME]"""
 import json
 import os
 import random
@@ -17,7 +20,7 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 import gen_golden  # noqa: E402
 import hostsim_util as hs  # noqa: E402
 from oracle import mask_ref  # noqa: E402
-from ref_answers import Answers, canon  # noqa: E402
+from ref_answers import Answers, canon, split_argv  # noqa: E402
 
 VOCAB = ["auth", "token", "tokens", "tokenizer", "secret", "secrets", "key", "keys", "api", "jwt", "pass", "password", "passwd", "pwd", "word", "phrase", "session", "id", "count",
          "status", "private", "client", "access", "refresh", "cookie", "x", "url", "ttl", "hash", "name", "type", "o", "oauth", "credential", "cred", "bearer", "signature", "sig",
@@ -42,26 +45,35 @@ def make_key(rng):
 
 
 def main() -> int:
-    record = "--record" in sys.argv
-    argv = [a for a in sys.argv[1:] if a != "--record"]
+    argv, record, device, name = split_argv(sys.argv[1:])
     seed = int(argv[0]) if len(argv) > 0 else 1
     nkeys = int(argv[1]) if len(argv) > 1 else 20000
     nbodies = int(argv[2]) if len(argv) > 2 else 2000
-    answers = Answers("mask", [seed, nkeys, nbodies], record)
+    answers = Answers("mask", [seed, nkeys, nbodies], record, name)
     if record:
         gen_golden.install_shims()
+    if device:
+        from mcp_context_forge_b200 import engine
+
+        ctx = engine.Context.get()
     ns = gen_golden.load_masking_twin() if record else None
     rng = random.Random(seed)
     t0 = time.time()
     bad = 0
     seen = set()
+    key_cases = []
     for _ in range(nkeys):
         k = make_key(rng)
         if k in seen:
             continue
         seen.add(k)
-        exp = answers(lambda: bool(ns["_is_sensitive_key"](k)))
-        got = hs.key_sensitive_host(k)
+        key_cases.append((k, answers(lambda: bool(ns["_is_sensitive_key"](k)))))
+    if device:
+        kb = [k.encode() for k, _ in key_cases]
+        kgot = engine.classify_keys_host(engine.Batch(ctx, sum(len(k) + 1 for k in kb), len(kb)), kb)
+    else:
+        kgot = [hs.key_sensitive_host(k) for k, _ in key_cases]
+    for (k, exp), got in zip(key_cases, kgot):
         orc = mask_ref.is_sensitive_key(k)
         if not (exp == got == orc):
             bad += 1
@@ -94,19 +106,37 @@ def main() -> int:
             return [rand_obj(depth - 1) for _ in range(rng.randint(0, 4))]
         return {rng.choice(keys): rand_obj(depth - 1) for _ in range(rng.randint(0, 6))}
 
-    nb = 0
+    body_cases = []
     for _ in range(nbodies):
         obj = rand_obj(rng.randint(1, 7))
         md = rng.choice([10, 10, 3, 1, 0, 2, 12, 5])
         exp = answers(lambda: ns["mask_sensitive_data"](obj, md))
         body = json.dumps(obj, ensure_ascii=rng.random() < 0.5, separators=rng.choice([(",", ":"), (", ", ": ")])).encode()
-        st, out = hs.mask_host(body, md)
+        body_cases.append((body, md, exp))
+    routes = [{}]
+    if device:                                                  # one launch per max_depth and route: cf_mask_host, and the fused cf_run_batch
+        routes = [{}, {}]
+        for md in sorted({md for _, md, _ in body_cases}):
+            idx = [i for i, c in enumerate(body_cases) if c[1] == md]
+            stream, offs = engine.pack_units([body_cases[i][0] for i in idx])
+            batch = engine.Batch(ctx, len(stream), len(idx))
+            st, outs = engine.mask_host(batch, stream, offs, md)
+            v, out, oo, _ = engine.run_batch(None, batch, stream, offs, engine.N.CF_STAGE_MASK, mask_max_depth=md)
+            for j, i in enumerate(idx):
+                routes[0][i] = (int(st[j]), outs[j])
+                routes[1][i] = (int(v["aux"][j]), out[int(oo[j]):int(oo[j + 1])].tobytes() if v["aux"][j] == engine.MASK_OK else None)
+    else:
+        routes[0] = {i: hs.mask_host(body, md) for i, (body, md, _) in enumerate(body_cases)}
+    nb = 0
+    for i, (body, md, exp) in enumerate(body_cases):
         orc = mask_ref.mask_json_bytes(body, md)
         nb += 1
-        if st != 0 or out != orc or json.loads(out) != exp:
-            bad += 1
-            if bad <= 10:
-                print("BODY", body[:300], md, "\n  reference", json.dumps(exp)[:300], "\n  kernel   ", st, (out or b"")[:300], "\n  oracle   ", orc[:300])
+        for route in routes:
+            st, out = route[i]
+            if st != 0 or out != orc or json.loads(out) != exp:
+                bad += 1
+                if bad <= 10:
+                    print("BODY", body[:300], md, "\n  reference", json.dumps(exp)[:300], "\n  kernel   ", st, (out or b"")[:300], "\n  oracle   ", orc[:300])
     # ---- the module a gateway imports (request_logging_masking_native_extension -> mcp_context_forge_b200/masking.py): its host logic (key
     # collection, cookie splitting, header walk, fallback probes) with the launches on the CPU simulator, against the twin's functions
     import importlib
@@ -115,7 +145,8 @@ def main() -> int:
 
     import hostsim_batcher
 
-    hostsim_batcher.install(pytest.MonkeyPatch())
+    if not device:
+        hostsim_batcher.install(pytest.MonkeyPatch())
     mod = importlib.import_module("request_logging_masking_native_extension")
     from mcp_context_forge_b200 import masking
 
@@ -152,7 +183,7 @@ def main() -> int:
             if bad <= 10:
                 print("FALLBACK", b_, "reference", repr(e_), "module", repr(g_))
     answers.finish()
-    print(f"seed={seed} keys={len(seen)} bodies={nb} module_calls={nm} bad={bad} time={time.time() - t0:.1f}s")
+    print(f"seed={seed} keys={len(seen)} bodies={nb} module_calls={nm} compared={len(seen) + nb + nm} bad={bad} time={time.time() - t0:.1f}s")
     return 1 if bad else 0
 
 

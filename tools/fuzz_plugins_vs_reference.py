@@ -3,8 +3,9 @@ order, payload rebuilding — on the engine's CPU simulator) against the REFEREN
 regex_filter, deny_filter, harmful_content_detector, sql_sanitizer, code_safety_linter, toon_encoder.  Random configurations (from pools that
 include rules matching "", group-reference templates, invalid patterns, IGNORECASE Unicode traps) and random payload shapes (nested dicts /
 lists / non-strings, every hook each plugin implements).  A configuration the engine rejects loudly (UnsupportedPattern) is skipped and counted.
-With --record the reference itself is run and its answers are stored (tools/ref_answers.py); without it they are read back from tests/golden/.
-usage: python tools/fuzz_plugins_vs_reference.py [seed] [rounds] [--record]"""
+With --record the reference itself is run and its answers are stored (tools/ref_answers.py); without it they are read back from tests/golden/
+(fuzz_plugins.json.gz, or NAME.json.gz with --answers NAME).  --device runs the plugins' launches on the GPU instead of the simulator.
+usage: python tools/fuzz_plugins_vs_reference.py [seed] [rounds] [--record | --device] [--answers NAME]"""
 import asyncio
 import json
 import os
@@ -17,7 +18,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 import gen_golden  # noqa: E402
-from ref_answers import Answers  # noqa: E402
+from ref_answers import Answers, split_argv  # noqa: E402
 
 WORDS = ["kill", "myself", "suicide", "self-harm", "want", "to", "die", "him", "her", "them", "someone", "shoot", "stab", "eradicate", "people", "racial", "slur", "hate", "speech", "crap",
          "crud", "innovative", "groundbreaking", "revolutionary", "the", "a", "of", "x", "Kill", "KILL", "ſuicide", "Kill", "é", "ß", "naïve", "日本語", "\U0001f600", "12", "_", "-", ".",
@@ -69,12 +70,11 @@ def norm(r):
 
 
 def main() -> int:
-    record = "--record" in sys.argv
-    argv = [a for a in sys.argv[1:] if a != "--record"]
+    argv, record, device, name = split_argv(sys.argv[1:])
     seed = int(argv[0]) if len(argv) > 0 else 1
     rounds = int(argv[1]) if len(argv) > 1 else 40
-    answers = Answers("plugins", [seed, rounds], record)
-    gen_golden.install_shims()
+    answers = Answers("plugins", [seed, rounds], record, name)
+    gen_golden.install_shims(reference=record)
     import pytest
     from cpex.framework import GlobalContext, PluginConfig, PluginContext, PromptPosthookPayload, PromptPrehookPayload, ToolPostInvokePayload, ToolPreInvokePayload
     if record:
@@ -96,7 +96,8 @@ def main() -> int:
     from mcp_context_forge_b200.plugins.toon_encoder import ToonEncoderPlugin
     from mcp_context_forge_b200.regex_frontend import UnsupportedPattern
 
-    hostsim_batcher.install(pytest.MonkeyPatch())
+    if not device:
+        hostsim_batcher.install(pytest.MonkeyPatch())
     ctx = PluginContext(global_context=GlobalContext(request_id="fuzz"))
     rng = random.Random(seed)
     loop = asyncio.new_event_loop()
@@ -172,7 +173,7 @@ def main() -> int:
                     if bad <= 6:
                         print("BAD stats", name, repr(cfg), exp, ours.get_stats())
     answers.finish()
-    print(f"seed={seed} rounds={rounds} hook_calls={n} configs_rejected_loudly={rejected} reference_raised={raised} bad={bad} time={time.time() - t0:.1f}s")
+    print(f"seed={seed} rounds={rounds} hook_calls={n} compared={n} configs_rejected_loudly={rejected} reference_raised={raised} bad={bad} time={time.time() - t0:.1f}s")
     return 1 if bad else 0
 
 

@@ -3,8 +3,13 @@ body csrc/json_tp.h on the 32-fibre warp emulator) against the REFERENCE'S OWN `
 /root/reference — no restatement in between (the oracle is compared too, so a gap in it shows).  Random JSON documents from the generator of
 tools/fuzz_toon_tp.py (adversarial keys / strings / numbers, tables, byte-level mutations).  orjson is not installable here: the strict stdlib
 parser stands in, and documents that would expose an orjson / json delta (integers beyond 64 bits, lone surrogates, non-finite floats) are skipped.
-With --record the reference itself is run and its answers are stored (tools/ref_answers.py); without it they are read back from tests/golden/.
-usage: python tools/fuzz_vs_reference.py [seed] [cases] [gen1|gen2|synth] [--record]"""
+With --record the reference itself is run and its answers are stored (tools/ref_answers.py); without it they are read back from tests/golden/
+(fuzz_toon.json.gz, or NAME.json.gz with --answers NAME).
+--device runs the compared documents as one batch through the CUDA kernels instead: cf_toon_host sequential (CF_TOON_SEQUENTIAL), token-parallel
+with hand-over (with and without CF_TOON_REPORT_ERRORS) and token-parallel alone (CF_TOON_NO_HANDOVER), and cf_run_batch(CF_STAGE_TOON), each
+against the reference's answer under the product's strictly-smaller rule.
+usage: python tools/fuzz_vs_reference.py [seed] [cases] [gen1|gen2|synth] [--record | --device] [--answers NAME]"""
+import ctypes
 import importlib.util
 import json
 import math
@@ -22,7 +27,7 @@ import hostsim_util as hs  # noqa: E402
 from fuzz_toon_tp import make_gen  # noqa: E402
 from mcp_context_forge_b200.plugins.toon_encoder import _encode_error  # noqa: E402
 from oracle import toon_ref  # noqa: E402
-from ref_answers import Answers  # noqa: E402
+from ref_answers import Answers, split_argv  # noqa: E402
 
 
 def load_reference_toon():
@@ -137,13 +142,64 @@ def make_gen2(rng):
     return case
 
 
+REPORT_ERRORS, SEQUENTIAL, NO_HANDOVER, HANDED_OVER, FB_NUM_EXACT = 1, 8, 16, 7, 1      # include/cfgpu.h CF_TOON_*, csrc/json_tp.h FB_*
+
+
+def device_toon(engine, texts, flags):
+    """cf_toon_host over `texts` as one batch: [(status, text or None)] and out_len (the hand-over reason under CF_TOON_NO_HANDOVER)."""
+    import numpy as np
+
+    ctx = engine.Context.get()
+    stream, offs = engine.pack_units(texts)
+    n = len(texts)
+    out = np.zeros(max(len(stream), 1), dtype=np.uint8)
+    out_len = np.zeros(n, dtype=np.uint32)
+    status = np.zeros(n, dtype=np.int32)
+    batch = engine.Batch(ctx, len(stream), n)                  # held for the call: the handle is freed with the object
+    ctx.check(ctx.lib.cf_toon_host(ctx.h, batch.h, flags, ctypes.cast(ctypes.c_char_p(stream), ctypes.c_void_p), len(stream),
+                                   offs.ctypes.data, n, out.ctypes.data, out_len.ctypes.data, status.ctypes.data), "cf_toon_host")
+    return [(int(s), out[int(o):int(o) + int(k)].tobytes().decode("utf-8", "surrogateescape") if s == 0 else None) for s, o, k in zip(status, offs, out_len)], out_len
+
+
+def device_run_batch(engine, texts, flags):
+    """cf_run_batch(CF_STAGE_TOON) over `texts`, the fused route the batched chain launches: [(status, text or None)]."""
+    ctx = engine.Context.get()
+    stream, offs = engine.pack_units(texts)
+    v, out, oo, _ = engine.run_batch(None, engine.Batch(ctx, len(stream), len(texts)), stream, offs, engine.N.CF_STAGE_TOON, toon_flags=flags)
+    return [(int(s), out[int(oo[i]):int(oo[i + 1])].tobytes().decode("utf-8", "surrogateescape") if s == 0 else None) for i, s in enumerate(v["aux"])]
+
+
+def device_checks(texts, smalls):
+    """Every device route against the reference's answer under the strictly-smaller rule: (bad, handed over, handed over for FB_NUM_EXACT).
+    With CF_TOON_REPORT_ERRORS status and text match exactly; without it the encoder may stop once the output has outgrown the input, so a
+    NOT_SMALLER / VALUE_ERROR / ATTR_ERROR answer may come back as any of the three (the stop_on_over contract)."""
+    from mcp_context_forge_b200 import engine
+
+    routes = [("sequential", device_toon(engine, texts, SEQUENTIAL | REPORT_ERRORS)[0], True),
+              ("token-parallel", device_toon(engine, texts, REPORT_ERRORS)[0], True),
+              ("token-parallel, errors not reported", device_toon(engine, texts, 0)[0], False),
+              ("cf_run_batch", device_run_batch(engine, texts, REPORT_ERRORS), True),
+              ("cf_run_batch, errors not reported", device_run_batch(engine, texts, 0), False)]
+    alone, why = device_toon(engine, texts, NO_HANDOVER | REPORT_ERRORS)
+    handed = [i for i, r in enumerate(alone) if r[0] == HANDED_OVER]
+    routes.append(("token-parallel without hand-over", [smalls[i] if r[0] == HANDED_OVER else r for i, r in enumerate(alone)], True))
+    bad = 0
+    for name, got, exact in routes:
+        for t, exp, g in zip(texts, smalls, got):
+            if g == exp or (not exact and exp[0] in (1, 3, 4) and g[0] in (1, 3, 4)):
+                continue
+            bad += 1
+            if bad <= 8:
+                print(f"BAD ({name})", repr(t)[:300], "\n   expected", repr(exp)[:200], "\n   device  ", repr(g)[:200])
+    return bad, len(handed), sum(1 for i in handed if why[i] == FB_NUM_EXACT)
+
+
 def main() -> int:
-    record = "--record" in sys.argv
-    argv = [a for a in sys.argv[1:] if a != "--record"]
+    argv, record, device, name = split_argv(sys.argv[1:])
     seed = int(argv[0]) if len(argv) > 0 else 1
     n = int(argv[1]) if len(argv) > 1 else 2000
     which = argv[2] if len(argv) > 2 else "gen1"
-    answers = Answers("toon", [seed, n, which], record)
+    answers = Answers("toon", [seed, n, which], record, name)
     toon = load_reference_toon() if record else None
     rng = random.Random(seed)
     if which == "synth":                                        # the bench's payload shapes (tabular / nested config / prose in JSON), 200 B .. 70 KB
@@ -156,7 +212,8 @@ def main() -> int:
     else:
         case = make_gen2(rng) if which == "gen2" else make_gen(rng)
     t0 = time.time()
-    done = skipped = handed = bad = worded = 0
+    done = skipped = handed = bad = worded = exact = 0
+    device_texts, device_smalls = [], []
     for it in range(n):
         t = case()
         r = answers(lambda: expected(toon, t))
@@ -165,11 +222,16 @@ def main() -> int:
             continue
         exp, message = (r[0], r[1]), r[2]
         done += 1
-        seq = hs.toon_host(t, unlimited=True)
-        tp = hs.toon_tp(t, unlimited=True, report_errors=True, order=(it & 1) | (rng.randrange(16) << 4))
-        if tp[0] == 7:
-            handed += 1
-            tp = exp
+        order = (it & 1) | (rng.randrange(16) << 4)
+        if device:                                              # the device has no unlimited output buffer: compared below, under the size rule
+            seq = tp = exp
+        else:
+            seq = hs.toon_host(t, unlimited=True)
+            tp = hs.toon_tp(t, unlimited=True, report_errors=True, order=order)
+            if tp[0] == HANDED_OVER:
+                handed += 1
+                exact += hs.toon_tp.last_reason == FB_NUM_EXACT
+                tp = exp
         try:
             orc = (0, toon_ref.encode(toon_ref.loads_strict(t)))
         except ValueError:
@@ -185,9 +247,14 @@ def main() -> int:
                     print("BAD MESSAGE", repr(t)[:400], "\n   reference", message, "\n   drop-in  ", msg)
         # the product's rule on top (include/cfgpu.h): the text is kept only when strictly smaller than the JSON it came from
         small = exp if (exp[0] != 0 or len(exp[1].encode("utf-8")) < len(t.encode("utf-8"))) else (1, None)
-        seq2, tp2 = hs.toon_host(t), hs.toon_tp(t, report_errors=True)
-        if tp2[0] == 7:
-            tp2 = small
+        if device:
+            device_texts.append(t)
+            device_smalls.append(small)
+            seq2 = tp2 = small
+        else:
+            seq2, tp2 = hs.toon_host(t), hs.toon_tp(t, report_errors=True)
+            if tp2[0] == HANDED_OVER:
+                tp2 = small
         if not (seq2 == small and tp2 == small):
             bad += 1
             if bad <= 8:
@@ -197,7 +264,11 @@ def main() -> int:
             if bad <= 8:
                 print("BAD", repr(t)[:400], "\n   reference", repr(exp)[:300], "\n   seq      ", repr(seq)[:300], "\n   tp       ", repr(tp)[:300], "\n   oracle   ", repr(orc)[:300])
     answers.finish()
-    print(f"seed={seed} cases={n} compared={done} skipped={skipped} handed_over={handed} error_messages_compared={worded} bad={bad} time={time.time() - t0:.1f}s")
+    if device:
+        b, handed, exact = device_checks(device_texts, device_smalls)
+        bad += b
+    print(f"seed={seed} cases={n} compared={done} skipped={skipped} handed_over={handed} handed_over_num_exact={exact} error_messages_compared={worded} bad={bad} "
+          f"time={time.time() - t0:.1f}s")
     return 1 if bad else 0
 
 

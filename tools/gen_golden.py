@@ -31,7 +31,8 @@ sys.path.insert(0, ROOT)
 OUT = os.path.join(ROOT, "tests", "golden")
 
 
-def install_shims():
+def install_shims(reference: bool = True):
+    """The stand-ins the reference's modules import; with `reference`, the reference's tree on sys.path too (only a recording needs it)."""
     from mcp_context_forge_b200.cpex_compat import install_as_cpex
 
     install_as_cpex(force=True)
@@ -67,7 +68,7 @@ def install_shims():
 
     ls.LoggingService = LoggingService
     sys.modules["mcpgateway.services.logging_service"] = ls
-    if REF not in sys.path:
+    if reference and REF not in sys.path:
         sys.path.insert(0, REF)
 
 

@@ -1,12 +1,13 @@
 """The reference's answers in a differential fuzz run, kept so that the run can be repeated without the reference's tree.
 
 `--record` (the reference's tree present): every answer is computed by the reference's own code, in call order, and the list is written
-to tests/golden/fuzz_<tool>.json.gz together with the run's arguments.  Otherwise the same seeded run reads the answers back in the same
+to tests/golden/fuzz_<tool>.json.gz (or tests/golden/<name>.json.gz) together with the run's arguments.  Otherwise the same seeded run reads the answers back in the same
 order.  Answers pass through JSON in both modes (tuples become lists), so both modes compare the same values; `canon` gives the product's
 side the same form."""
 import gzip
 import json
 import os
+from typing import Optional
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -16,8 +17,8 @@ def canon(v):
 
 
 class Answers:
-    def __init__(self, tool: str, args, record: bool):
-        self.path = os.path.join(ROOT, "tests", "golden", f"fuzz_{tool}.json.gz")
+    def __init__(self, tool: str, args, record: bool, name: Optional[str] = None):
+        self.path = os.path.join(ROOT, "tests", "golden", f"{name or 'fuzz_' + tool}.json.gz")
         self.args = [str(a) for a in args]
         self.live = record
         self.i = 0
@@ -48,3 +49,19 @@ class Answers:
             print(f"wrote {self.path}: {os.path.getsize(self.path)} bytes")
         elif self.i != len(self.values):
             raise SystemExit(f"{self.path}: {len(self.values) - self.i} recorded answers were not asked for (the generator changed: record again)")
+
+
+def split_argv(argv):
+    """(positional arguments, --record, --device, --answers NAME) of a fuzz tool's command line."""
+    rest, name, i = [], None, 0
+    while i < len(argv):
+        if argv[i] == "--answers":
+            name = argv[i + 1]
+            i += 2
+            continue
+        rest.append(argv[i])
+        i += 1
+    record, device = "--record" in rest, "--device" in rest
+    if record and device:
+        raise SystemExit("--record runs the reference's tree, --device runs without it: pick one")
+    return [a for a in rest if a not in ("--record", "--device")], record, device, name
