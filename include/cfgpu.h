@@ -110,6 +110,7 @@ uint32_t cf_prog_patterns(const cf_prog* p);
 
 /* ---------------- batches (device-resident packed streams) ---------------- */
 int cf_batch_create(cf_ctx* ctx, uint64_t max_stream_bytes, uint32_t max_units, cf_batch** out);
+/* a freed handle is recycled: the next cf_batch_create may return the same pointer, so never compare a live handle with a freed one */
 void cf_batch_free(cf_batch* b);
 /* async H2D of a packed stream on `cuda_stream` (cudaStream_t, may be NULL) */
 int cf_batch_upload(cf_ctx* ctx, cf_batch* b, const uint8_t* stream, uint64_t stream_bytes,

@@ -16,6 +16,8 @@
 #include <string.h>
 
 #include <atomic>
+#include <mutex>
+#include <new>
 #include <string>
 #include <vector>
 
@@ -1102,10 +1104,41 @@ uint32_t cf_prog_patterns(const cf_prog* p) { return p ? p->npat : 0; }
 
 static uint64_t ntiles_for(uint64_t nbytes, uint32_t tile) { return (nbytes + 2 + tile - 1) / tile; }
 
+// Freed batch handles are kept (up to BATCH_POOL of them) and handed out again, the last freed first: a batch created right after
+// another was freed takes its address.  Whatever is keyed on a batch handle must therefore key on cf_batch::generation as well
+// (cf_sub_host's copy of the offsets does).  The pool is never destroyed, so a handle freed during process exit still finds it.
+static const size_t BATCH_POOL = 16;
+static std::mutex& batch_pool_mu() { static std::mutex* m = new std::mutex; return *m; }
+static std::vector<cf_batch*>& batch_pool() { static std::vector<cf_batch*>* v = new std::vector<cf_batch*>; return *v; }
+
+static cf_batch* batch_alloc() {
+  {
+    std::lock_guard<std::mutex> g(batch_pool_mu());
+    std::vector<cf_batch*>& pool = batch_pool();
+    if (!pool.empty()) {
+      cf_batch* b = pool.back();
+      pool.pop_back();
+      return new (b) cf_batch();
+    }
+  }
+  return new (std::nothrow) cf_batch();
+}
+
+static void batch_release(cf_batch* b) {
+  b->~cf_batch();
+  {
+    std::lock_guard<std::mutex> g(batch_pool_mu());
+    std::vector<cf_batch*>& pool = batch_pool();
+    if (pool.size() < BATCH_POOL) { pool.push_back(b); return; }
+  }
+  if (alignof(cf_batch) > __STDCPP_DEFAULT_NEW_ALIGNMENT__) ::operator delete(b, std::align_val_t(alignof(cf_batch)));
+  else ::operator delete(b);
+}
+
 int cf_batch_create(cf_ctx* ctx, uint64_t max_stream_bytes, uint32_t max_units, cf_batch** out) {
   if (!ctx || !out) return CF_E_BADARG;
   CF_CUDA(ctx, cudaSetDevice(ctx->device));
-  cf_batch* b = new (std::nothrow) cf_batch();
+  cf_batch* b = batch_alloc();
   if (!b) return CF_E_NOMEM;
   b->ctx = ctx;
   *out = b;
@@ -1153,7 +1186,7 @@ void cf_batch_free(cf_batch* b) {
   cudaFree(b->d_buf);
   cudaFree(b->d_offsets);
   cudaFree(b->d_coarse);
-  delete b;
+  batch_release(b);
 }
 
 uint32_t cf_batch_units(const cf_batch* b) { return b ? b->n : 0; }

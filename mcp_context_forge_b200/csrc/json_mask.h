@@ -123,13 +123,17 @@ struct KeyClassifier {
   }
 };
 
+// A key parsed from JSON carries JF_ESC when its text holds escapes; a raw key name (cf_classify_keys_host) never does, so a
+// backslash in it is a character of the name.  Only ASCII letters and digits count, so the raw bytes of a multi-byte character
+// classify like the character itself (a run of non-alphanumerics is one separator either way).
 CF_HD bool key_sensitive(const uint8_t* s, const JNode& key) {
   KeyClassifier kc;
   kc.init();
   StrIter it{s + key.off, s + key.off + key.len};
+  const bool esc = (key.t & cfj::JF_ESC) != 0;
   bool prev_lower_or_digit = false, prev_us = false;
   while (!it.done()) {
-    const uint32_t ch = it.next();
+    const uint32_t ch = esc ? it.next() : *it.p++;
     const bool is_upper = ch >= 'A' && ch <= 'Z';
     const bool is_lower = ch >= 'a' && ch <= 'z';
     const bool is_digit = ch >= '0' && ch <= '9';

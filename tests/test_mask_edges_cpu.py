@@ -72,3 +72,16 @@ def test_module_batches_on_the_simulator(mod):
         mod.mask_sensitive_json_bytes(b'{"password":1e400}')
     with pytest.raises(RuntimeError, match="3200-bit"):
         mod.mask_sensitive_json_bytes_batch([b"[1.5]", b"[0." + b"1" * 1200 + b"]"])
+
+
+def test_backslash_key_names_are_classified_as_written():
+    """A raw key name's backslash is a character, not an escape (regression: "pass\\word" was classified as "password"); the same
+    names escaped in a JSON body are decoded first."""
+    from oracle import mask_ref
+
+    for k in tg.BACKSLASH_KEYS:
+        assert hs.key_sensitive_host(k) == mask_ref.is_sensitive_key(k), k
+    assert any(mask_ref.is_sensitive_key(k) for k in tg.BACKSLASH_KEYS) and not all(mask_ref.is_sensitive_key(k) for k in tg.BACKSLASH_KEYS)
+    import json
+
+    check([json.dumps({k: "v", "n": [k]}).encode() for k in tg.BACKSLASH_KEYS], 10)

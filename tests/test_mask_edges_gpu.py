@@ -10,6 +10,7 @@ usually goes wrong:
 Every case runs through the drop-in module's batch API and through cf_run_batch(SCAN | MASK) with host buffers and resident.
 tests/test_mask_edges_cpu.py runs the same bodies on the host build of csrc/json_mask.h."""
 import importlib
+import json
 import math
 import random
 
@@ -112,6 +113,13 @@ def expected(body: bytes, max_depth: int):
         return None
 
 
+# Key names holding a backslash or the text of a JSON escape.  A name handed over as a str (mask_sensitive_data, the header
+# masking) is classified as written: "pass\\word" is not "password", and "pass\\u0077ord" is not either.  In a JSON body the
+# same names arrive escaped and are decoded first.
+BACKSLASH_KEYS = ["pass\\word", "pass\\\\word", "\\password", "password\\", "api\\_key", "API\\u004bey", "pass\\u0077ord", "to\\ken",
+                  "secret\\n", "\\u0074oken", "jwt\\", "\\", "x\\", "\\\"token", "pass\\/word", "to\\u006ben"]
+
+
 def packed_with_neighbours(special, n_plain: int = 3000, seed: int = 7):
     """`special` bodies at random places among n_plain ordinary synth bodies (several to a warp once the batch is this large)."""
     rng = random.Random(seed)
@@ -202,3 +210,11 @@ def test_outputs_much_larger_than_their_input_among_packed_neighbours(mod, chain
 def test_literals_beyond_the_workspace_fail_loudly(mod):
     with pytest.raises(RuntimeError, match="3200-bit"):
         mod.mask_sensitive_json_bytes_batch([b"[1.5]", b"[0." + b"1" * 1200 + b"]"])
+
+
+def test_backslash_key_names_are_classified_as_written(mod):
+    data = {k: "v" for k in BACKSLASH_KEYS}
+    assert mod.mask_sensitive_data(data) == mask_ref.mask_value(data)
+    assert mod.mask_sensitive_headers(data) == mask_ref.mask_headers(data)
+    bodies = [json.dumps({k: "v"}).encode() for k in BACKSLASH_KEYS]
+    assert mod.mask_sensitive_json_bytes_batch(bodies) == [expected(b, 10) for b in bodies]
