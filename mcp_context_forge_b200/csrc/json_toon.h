@@ -649,15 +649,18 @@ enum : int {
   TS_ATTR_ERROR = 4 /* the reference's unchecked .keys() */, TS_UNSUPPORTED = 6
 };
 
+// n counts every byte of the text (saturating at 2^32 - 1); only the first cap of them are stored.  Whether the text fits is
+// decided on its final length, not on the most bytes written along the way: a columnar header takes back whitespace it has
+// already written (HeaderSink), and what it keeps before that whitespace was stored whenever the final length fits.
 struct Out {
   uint8_t* p;
   uint32_t n, cap;
-  bool over;
-  CF_HD void put(uint32_t c) { if (n < cap) p[n++] = (uint8_t)c; else over = true; }
+  CF_HD bool over() const { return n > cap; }
+  CF_HD void put(uint32_t c) { if (n < cap) p[n] = (uint8_t)c; n += n != 0xFFFFFFFFu; }
   // copy a span of source bytes; the in-capacity case is unrolled so that a lone GPU thread has
   // several independent loads in flight
   CF_HD void put_span(const uint8_t* b, uint32_t len) {
-    if (n + len <= cap) {
+    if (n <= cap && len <= cap - n) {
       uint8_t* d = p + n;
       uint32_t i = 0;
       for (; i + 4 <= len; i += 4) {
@@ -692,7 +695,8 @@ struct Ctx {
   int err;          // 0 or TS_VALUE_ERROR / TS_ATTR_ERROR / TS_UNSUPPORTED
   bool started;     // a line has been opened already (next line needs a '\n' first)
   bool stop_on_over; // give up as soon as the output cannot be smaller (errors then go unreported: fine when
-                    // the caller treats encode errors and "not smaller" alike, i.e. skip_on_error=True)
+                    // the caller treats encode errors and "not smaller" alike, i.e. skip_on_error=True).  Checked only
+                    // between rows and between frames, where every header is complete: no take-back can follow there
   Big* big;         // workspace for the exact number path
   uint8_t* digits;  // decimal digit workspace
   uint32_t digits_cap;
@@ -765,7 +769,7 @@ struct HeaderSink {
   CF_HD void cp(uint32_t x) {
     if (x == '\n') {
       if (strip) {
-        if (piece && !c.out.over) c.out.n -= ws_tail;             // rstrip of the line that ends here
+        if (piece) c.out.n -= ws_tail;                             // rstrip of the line that ends here
         c.out.put('\n'); c.out.spaces(row_pre);
       } else { c.out.put('\n'); c.out.spaces(hdr_pre); }
       ++piece; ws_tail = 0; at_start = true;
@@ -1019,7 +1023,7 @@ CF_HD void emit_columnar(Ctx& c, uint32_t arr, uint32_t row_pre, bool aligned, u
   bool f0 = true;
   for (uint32_t k = N[first].off; k; k = N[k].next) { if (!f0) hs.cp(','); f0 = false; hs.key(N[k]); }
   hs.cp('}'); hs.cp(':');
-  for (uint32_t x = first; x && !c.err && !(c.out.over && c.stop_on_over); x = N[x].next) {
+  for (uint32_t x = first; x && !c.err && !(c.out.over() && c.stop_on_over); x = N[x].next) {
     newline(c, row_pre);
     bool f1 = true;
     if (aligned) {
@@ -1078,7 +1082,7 @@ CF_HD void toon_emit(Ctx& c, uint32_t root) {
   if (rk != J_ARR && rk != J_OBJ) { emit_prim(c, root); return; }
   if (rk == J_ARR) { c.started = true; begin_array(c, root, 0, 0, st, &sp); }
   else { if (N[root].len == 0) return; st[sp++] = Frame{FR_OBJ, root, N[root].off, 0, 0, 0}; }
-  while (sp > 0 && !c.err && !(c.out.over && c.stop_on_over)) {
+  while (sp > 0 && !c.err && !(c.out.over() && c.stop_on_over)) {
     Frame& f = st[sp - 1];
     if (f.cur == 0) { --sp; continue; }
     if (f.kind == FR_OBJ) {                                   // toon.py:514-565
@@ -1156,12 +1160,12 @@ CF_HD int toon_finish(int pr, const uint8_t* s, const JNode* nodes, uint8_t* out
   if (pr == PARSE_UNSUPPORTED) return TS_UNSUPPORTED;
   Ctx c;
   c.s = s; c.nodes = nodes;
-  c.out.p = out; c.out.n = 0; c.out.cap = out_cap; c.out.over = false;
+  c.out.p = out; c.out.n = 0; c.out.cap = out_cap;
   c.err = 0; c.started = false; c.stop_on_over = stop_on_over;
   c.big = big; c.digits = digits; c.digits_cap = digits_cap;
   toon_emit(c, 0);
   if (c.err) return c.err;
-  if (c.out.over) return TS_NOT_SMALLER;
+  if (c.out.over()) return TS_NOT_SMALLER;
   *out_len = c.out.n;
   return TS_CONVERTED;
 }

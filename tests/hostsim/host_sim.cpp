@@ -147,12 +147,14 @@ int cfh_sub(cf_builder* b, uint32_t ordered_index, const uint8_t* unit, uint64_t
 
 // ---- TOON: run the shared json_toon.h pipeline on the CPU (same code the CUDA kernel calls) ----
 #include "../../mcp_context_forge_b200/csrc/json_toon.h"
-extern "C" int cfh_toon(const uint8_t* text, uint32_t n, uint8_t* out, uint32_t out_cap, uint32_t* out_len) {
+// stop_on_over: give up at the first check past the capacity, as toon_kernel does without CF_TOON_REPORT_ERRORS
+extern "C" int cfh_toon(const uint8_t* text, uint32_t n, uint8_t* out, uint32_t out_cap, uint32_t* out_len, int stop_on_over) {
   std::vector<cfj::JNode> nodes(n / 2 + 4);
   cfj::Big big;
   std::vector<uint8_t> digits(1240);
   *out_len = 0;
-  return cfj::toon_process(text, n, nodes.data(), (uint32_t)nodes.size(), out, out_cap, out_len, &big, digits.data(), (uint32_t)digits.size(), false);
+  return cfj::toon_process(text, n, nodes.data(), (uint32_t)nodes.size(), out, out_cap, out_len, &big, digits.data(), (uint32_t)digits.size(),
+                           stop_on_over != 0);
 }
 
 // ---- masking: shared json_mask.h pipeline on the CPU ----

@@ -120,17 +120,21 @@ class HostProgram:
 TOON_STATUS = {0: "converted", 1: "not_smaller", 2: "not_json", 3: "value_error", 4: "attr_error", 6: "unsupported"}
 
 
-def toon_host(text: str, unlimited: bool = False, indexed: bool = False):
+def toon_host(text: str, unlimited: bool = False, indexed: bool = False, stop_on_over: bool = False):
     """(status, toon_text_or_None) from the shared json_toon.h pipeline compiled for the CPU.
     unlimited=True lifts the product's "strictly smaller" capacity so the encoder output itself can
     be compared with the reference's toon.encode.  indexed=True parses through the structural index +
-    token-driven builder (json_index.h — the path the CUDA kernels take) instead of the sequential parser."""
+    token-driven builder (json_index.h — the path the CUDA kernels take) instead of the sequential parser.
+    stop_on_over=True (sequential parser only) gives up once the output is past the capacity, as toon_kernel does when errors
+    are not reported."""
     b = text if isinstance(text, bytes) else text.encode("utf-8", "surrogatepass")
     cap = len(b) * 6 + 4096 if unlimited else max(len(b) - 1, 0)
     out = ctypes.create_string_buffer(max(cap, 1))
     n = ctypes.c_uint32()
-    fn = lib().cfh_toon_indexed if indexed else lib().cfh_toon
-    st = fn(b, len(b), out, cap, ctypes.byref(n))
+    if indexed:
+        st = lib().cfh_toon_indexed(b, len(b), out, cap, ctypes.byref(n))
+    else:
+        st = lib().cfh_toon(b, len(b), out, cap, ctypes.byref(n), 1 if stop_on_over else 0)
     return st, (out.raw[: n.value].decode("utf-8", "surrogatepass") if st == 0 else None)
 
 

@@ -61,6 +61,7 @@ def test_outputs_much_larger_than_their_input():
         else:
             assert (st, first) == (0, e)
         assert hs.mask_host(b, md) == (0, e)
+    assert {len(tg.expected(b, md)) - 5 * len(b) for b, md in tg.growth_cases()} >= {32, 33}
 
 
 def test_module_batches_on_the_simulator(mod):

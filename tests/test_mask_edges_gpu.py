@@ -6,7 +6,8 @@ usually goes wrong:
   * values that are never printed — numbers out of binary64's range and lone surrogates under a sensitive key, below the depth cap,
     overwritten by a duplicate key: serde_json parses the whole document first, so each one fails the call;
   * nesting at 64 .. 200 levels, either side of serde_json's limit of 127;
-  * outputs up to ten times their input, beside thousands of ordinary bodies packed several to a warp.
+  * outputs up to ten times their input, and ones exactly as large as the first pass's room (5 * len + 32 bytes) or one byte
+    larger, beside thousands of ordinary bodies packed several to a warp.
 Every case runs through the drop-in module's batch API and through cf_run_batch(SCAN | MASK) with host buffers and resident.
 tests/test_mask_edges_cpu.py runs the same bodies on the host build of csrc/json_mask.h."""
 import importlib
@@ -101,9 +102,19 @@ GROWTH_SHAPES = [("0", lambda s: "[" + s + "]", 1), ("0", lambda s: "[" * 10 + s
                  ("1e15", lambda s: "[" + s + "]", 10), ("-0", lambda s: "[" + s + "]", 10)]
 
 
+def exact_room_cases():
+    """(body, max_depth) pairs whose output is exactly the room of mask_kernel's first pass (5 * len + 32 bytes) or one byte more:
+    at max_depth 2 each 0 of '{"k":[0,...]}' prints as "<nested too deep>", and trailing spaces set the input length."""
+    out = []
+    for m in (6, 40, 800):
+        for key, extra in (("k", 0), ("kk", 1)):
+            out.append((('{"%s":[%s]}' % (key, ",".join(["0"] * m)) + " " * (2 * m - 12 - extra)).encode(), 2))
+    return out
+
+
 def growth_cases():
-    """(body, max_depth) pairs: every shape at every size."""
-    return [(_fill(e, size, w).encode(), md) for e, w, md in GROWTH_SHAPES for size in GROWTH_SIZES]
+    """(body, max_depth) pairs: every shape at every size, and the bodies that fill the first pass's room exactly."""
+    return [(_fill(e, size, w).encode(), md) for e, w, md in GROWTH_SHAPES for size in GROWTH_SIZES] + exact_room_cases()
 
 
 def expected(body: bytes, max_depth: int):
@@ -204,6 +215,7 @@ def test_outputs_much_larger_than_their_input_among_packed_neighbours(mod, chain
         bodies, where = packed_with_neighbours(special, seed=md)
         exp = check_all_paths(mod, chain, bodies, md)
         assert any(len(exp[i]) > 5 * len(bodies[i]) + 32 for i in where)      # outgrows the room of the first pass
+    assert {len(expected(b, md)) - 5 * len(b) for b, md in cases} >= {32, 33}   # fills it exactly, and by one byte more
     assert max(len(expected(b, md)) / len(b) for b, md in cases) > 9
 
 
