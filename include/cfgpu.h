@@ -254,7 +254,8 @@ typedef struct cf_verdict {
 int cf_run_batch(cf_ctx* ctx, cf_prog* prog /* may be NULL without SCAN/SUB */, cf_batch* b, const uint8_t* stream, uint64_t stream_bytes,
                  const uint64_t* offsets, uint32_t n_units, uint32_t stage_mask, const uint8_t* unit_stages, uint32_t toon_flags, int mask_max_depth,
                  cf_verdict* verdicts, uint64_t* bitmaps_full, uint8_t* out_bytes, uint64_t out_cap, uint64_t* out_offsets, uint64_t* out_needed);
-/* the device buffer of the last CF_RUN_OUTPUTS_RESIDENT call of this ctx (valid until the next cf_run_batch / *_host call) */
+/* the device buffer of the last CF_RUN_OUTPUTS_RESIDENT call of this ctx (valid until the next cf_run_batch, cf_mask_host or
+ * cf_toon_host call on it: those gather into the same buffer) */
 int cf_run_batch_device_output(cf_ctx* ctx, const uint8_t** d_out, uint64_t* bytes);
 /* synchronous copy of `bytes` device bytes to a host buffer (for callers without a CUDA runtime binding of their own) */
 int cf_copy_to_host(cf_ctx* ctx, void* host_dst, const void* device_src, uint64_t bytes);
@@ -270,8 +271,9 @@ int cf_copy_to_host(cf_ctx* ctx, void* host_dst, const void* device_src, uint64_
  * ctx can be in flight at once on different streams.  Memory of a run: 8 x max_stream_bytes of TOON scratch, max_stream_bytes of
  * TOON output, about 170 bytes per unit, 8 MiB of scan queue and the arena.  cf_run_set_mask adds the masking workspace: 7 x
  * max_stream_bytes + 52 bytes per unit (the first pass's room of 5 len + 32 bytes per unit, and the parser's node index; its nodes
- * are the TOON scratch).  (The run cf_run_batch uses borrows the context's TOON and masking workspaces instead, the ones cf_toon
- * uses, so a context holds one.)
+ * are the TOON scratch).  (The context's own run, the one cf_run_batch, cf_toon and cf_toon_host use, is grown with their batches and
+ * takes its TOON workspace on the first call that needs TOON or masking and its masking workspace on the first masking call, so a
+ * context that only scans and rewrites holds neither, and any context holds at most one of each.)
  *
  * cf_run_enqueue: the batch must be resident (cf_batch_upload on the same stream, or ordered before it).  d_verdicts (n_units
  * records), d_out_offsets (n_units + 1), d_out (out_cap bytes), d_bitmaps_full (n_units * W words; required with SCAN or SUB) and

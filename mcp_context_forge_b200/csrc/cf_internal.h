@@ -36,18 +36,30 @@ struct cf_ctx {
   uint32_t qphase = 0;
   uint64_t* d_queue = nullptr;      // candidate start positions
   uint32_t qcap = 1u << 20;
-  void* d_toon_scratch = nullptr;   // DOM node arrays for toon_kernel (grown on demand)
-  uint64_t toon_scratch_bytes = 0;
-  struct DevBuf { void* p = nullptr; size_t cap = 0; };
-  DevBuf tmp[16];                   // grow-only device scratch of the *_host entry points (no cudaMalloc per call)
+  // grow-only device scratch of the synchronous entry points (cf_dev_reserve: no cudaMalloc per call), freed with the context
+  struct DevBuf {
+    void* p = nullptr;
+    size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { cudaFree(p); }
+  };
+  // cf_sub_device (cf_sub_host, and cf_run_finish's deferred units): the rewritten texts, a pass's descriptors (soff | bound | sel),
+  // its records and the Pike VM's capture words
+  DevBuf sub_scratch, sub_desc, sub_rec, sub_pike;
+  DevBuf sub_out_offsets, sub_out;  // cf_sub_host's gather of the rewritten texts
+  DevBuf verdicts, unit_stages;     // cf_run_batch with host buffers: verdict records, per-unit stage masks on the way in
+  // the gather of cf_run_batch and of cf_toon_host: out offsets and the gathered texts.  Shared, as neither call's texts outlive it,
+  // except `gathered` after a CF_RUN_OUTPUTS_RESIDENT cf_run_batch: cf_run_batch_device_output hands it out until either call runs again
+  DevBuf out_offsets, gathered;
+  DevBuf bitmaps;                   // pattern bitmaps of cf_scan_host and cf_run_batch, or cf_classify_keys_host's flags
   DevBuf d_tok, d_ntok;             // structural index of the current batch (json_index_kernel)
-  DevBuf toon_order;                // TOON first pass: units in cost order (uint32 per unit)
-  DevBuf toon_sort;                 // ... and the sort behind it: unit indices | keys in | keys out | radix-sort temp storage
   void* h_stage = nullptr;          // pinned host staging for gathered results
   size_t h_stage_bytes = 0;
   const uint8_t* run_out = nullptr;   // device buffer of the last CF_RUN_OUTPUTS_RESIDENT call
   uint64_t run_out_bytes = 0;
-  cf_run* run = nullptr;              // cf_run_batch's run (legacy stream), grown with the batches
+  cf_run* run = nullptr;              // the run of cf_run_batch, cf_toon and cf_toon_host (ctx_run in cfjson.cu), grown with the batches
   // optional per-launch timing of the dominant kernel (bench.py roofline): event pairs
   std::vector<cudaEvent_t> prof_ev;
   uint32_t prof_used = 0;
@@ -124,9 +136,10 @@ int cf_dev_reserve(cf_ctx* ctx, cf_ctx::DevBuf& b, size_t need);
 int cf_stage_reserve(cf_ctx* ctx, size_t need);
 
 // regex_filter substitution of the selected units on stream `st` (cfgpu.cu); the rewritten texts stay on the device.  Unit units[i]
-// ends as rec[2i+1] bytes at ctx->tmp[8] + rec[2i], or as the unit itself in the batch's stream when rec[2i] == ~0 (no rule changed
-// it).  h_offsets: host copy of the batch's offsets (scratch sizing); h_stage: pinned, cf_sub_stage_bytes(n_sel) bytes, and *rec
-// points into it.  Returns with the work on `st` done.  Only the scratch tmp[8..15] is written.
+// ends as rec[2i+1] bytes at ctx->sub_scratch.p + rec[2i], or as the unit itself in the batch's stream when rec[2i] == ~0 (no rule
+// changed it).  h_offsets: host copy of the batch's offsets (scratch sizing); h_stage: pinned, cf_sub_stage_bytes(n_sel) bytes, and
+// *rec points into it.  Returns with the work on `st` done.  Of the context's device buffers only sub_scratch, sub_desc, sub_rec and
+// sub_pike are written.
 size_t cf_sub_stage_bytes(uint32_t n_sel);
 int cf_sub_device(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint64_t* h_offsets, const uint32_t* units, uint32_t n_sel, cudaStream_t st,
                   uint8_t* h_stage, const uint64_t** rec);
@@ -159,7 +172,7 @@ struct cf_run {
   uint64_t* d_queue = nullptr;                          // scan candidate queue and its counters
   uint64_t* d_qstate = nullptr;
   uint32_t qphase = 0;
-  void* d_toon_scratch = nullptr;                       // TOON: token / DOM scratch, unit order and its sort
+  void* d_toon_scratch = nullptr;                       // TOON workspace (run_reserve_toon): token / DOM scratch, unit order and its sort
   uint64_t toon_scratch_bytes = 0;
   uint32_t* d_toon_order = nullptr;
   uint8_t* d_toon_sort = nullptr;
@@ -233,6 +246,8 @@ __device__ __forceinline__ void warp_copy_span(uint8_t* out, uint64_t at, const 
 
 // the scan of cf_scan on a given candidate queue / counter pair (cfgpu.cu)
 int cf_scan_launch(cf_ctx* ctx, cf_prog* p, cf_batch* b, uint64_t* d_bitmaps, cudaStream_t st, uint64_t* queue, uint64_t* qstate, uint32_t* qphase);
+// cf_init's share of cfjson.cu: allows toon_tp_kernel its dynamic shared memory on the current device
+cudaError_t cf_toon_tp_allow_smem();
 // cf_run_enqueue's substitution on `st` (cfgpu.cu): dirty-unit selection, bounds and arena allocation, then the sub_kernel launches
 int cf_sub_enqueue(cf_ctx* ctx, cf_prog* p, cf_batch* b, cf_run* run, const uint64_t* d_bitmaps, const uint8_t* d_unit_stages, cudaStream_t st);
 

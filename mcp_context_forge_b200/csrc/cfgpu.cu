@@ -851,9 +851,9 @@ static int upload_dfa(cf_ctx* ctx, const cfre::DfaOut& d, DevDfa& o) {
 }
 
 // ---- the substitution pass shared by cf_sub_host and cf_run_batch (cf_internal.h)
-// Descriptors of a pass, one H2D from pinned staging into tmp[9]: soff[n] | bound[n] | sel[n]; then rec[2n] comes back in one D2H.
+// Descriptors of a pass, one H2D from pinned staging into ctx->sub_desc: soff[n] | bound[n] | sel[n]; then rec[2n] comes back in one D2H.
 static size_t sub_desc_bytes(uint32_t n) { return ((size_t)n * 20 + 15) & ~(size_t)15; }
-static const uint32_t* sub_desc_sel(const cf_ctx* ctx, uint32_t n) { return (const uint32_t*)((const uint64_t*)ctx->tmp[9].p + 2 * (size_t)n); }
+static const uint32_t* sub_desc_sel(const cf_ctx* ctx, uint32_t n) { return (const uint32_t*)((const uint64_t*)ctx->sub_desc.p + 2 * (size_t)n); }
 size_t cf_sub_stage_bytes(uint32_t n_sel) { return sub_desc_bytes(n_sel) + (size_t)n_sel * 16; }
 
 // the sub_kernel launches of one pass: SUB_LAUNCH_RULES rules per launch; each further launch continues every unit from the record
@@ -927,28 +927,28 @@ int cf_sub_device(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint64_t* h_offset
   }
   int rc;
   // grow-only scratch of the context: no cudaMalloc / cudaFree per call
-  if ((rc = cf_dev_reserve(ctx, ctx->tmp[9], sub_desc_bytes(n_sel))) || (rc = cf_dev_reserve(ctx, ctx->tmp[12], (size_t)n_sel * 16))) return rc;
-  uint64_t* d_desc = (uint64_t*)ctx->tmp[9].p;
+  if ((rc = cf_dev_reserve(ctx, ctx->sub_desc, sub_desc_bytes(n_sel))) || (rc = cf_dev_reserve(ctx, ctx->sub_rec, (size_t)n_sel * 16))) return rc;
+  uint64_t* d_desc = (uint64_t*)ctx->sub_desc.p;
   SubParams SP;
   SP.stream = b->d_buf + cf::FRONT_PAD;
   SP.offsets = b->d_offsets;
   SP.soff = d_desc; SP.bound = d_desc + n_sel; SP.sel = sub_desc_sel(ctx, n_sel);
-  SP.rec = (uint64_t*)ctx->tmp[12].p;
+  SP.rec = (uint64_t*)ctx->sub_rec.p;
   SP.n_sel = n_sel;
   SP.n_dev = nullptr;
   SP.pike = nullptr; SP.pike_words = p->pike_words;
   if (SP.pike_words) {
     if ((uint64_t)n_sel * SP.pike_words * 4 > (4ull << 30)) { ctx->err = "capture scratch exceeds 4 GiB (too many units for a rule with group references)"; return CF_E_CAPACITY; }
-    if ((rc = cf_dev_reserve(ctx, ctx->tmp[15], (size_t)n_sel * SP.pike_words * 4))) return rc;
-    SP.pike = (uint32_t*)ctx->tmp[15].p;
+    if ((rc = cf_dev_reserve(ctx, ctx->sub_pike, (size_t)n_sel * SP.pike_words * 4))) return rc;
+    SP.pike = (uint32_t*)ctx->sub_pike.p;
   }
   for (bool again = true; again;) {        // one pass, and another while some unit outgrew a bound below its worst case
     again = false;
     uint64_t total = 0;
     for (uint32_t i = 0; i < n_sel; ++i) { soff[i] = total; total += 2 * bound[i]; }
     if (total > (8ull << 30)) { ctx->err = "substitution scratch exceeds 8 GiB"; return CF_E_CAPACITY; }
-    if ((rc = cf_dev_reserve(ctx, ctx->tmp[8], total))) return rc;
-    SP.scratch = (uint8_t*)ctx->tmp[8].p;
+    if ((rc = cf_dev_reserve(ctx, ctx->sub_scratch, total))) return rc;
+    SP.scratch = (uint8_t*)ctx->sub_scratch.p;
     CF_CUDA(ctx, cudaMemcpyAsync(d_desc, h_stage, sub_desc_bytes(n_sel), cudaMemcpyHostToDevice, st));
     if ((rc = sub_launch_rules(ctx, p, SP, st))) return rc;
     CF_CUDA(ctx, cudaMemcpyAsync(rec, SP.rec, (size_t)n_sel * 16, cudaMemcpyDeviceToHost, st));
@@ -991,6 +991,7 @@ int cf_init(int device_ordinal, cf_ctx** out) {
   if (const char* e = getenv("CF_SCAN_RESERVE_SMS")) ctx->scan_reserve_sms = (uint32_t)atoi(e);
   CF_CUDA(ctx, cudaFuncSetAttribute(scan_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SCAN_SMEM));
   CF_CUDA(ctx, cudaFuncSetAttribute(scan_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SCAN_SMEM));
+  CF_CUDA(ctx, cf_toon_tp_allow_smem());
   return CF_OK;
 }
 
@@ -999,13 +1000,9 @@ void cf_shutdown(cf_ctx* ctx) {
   cudaSetDevice(ctx->device);
   cudaFree(ctx->d_qstate);
   cudaFree(ctx->d_queue);
-  cudaFree(ctx->d_toon_scratch);
-  for (auto& t : ctx->tmp) cudaFree(t.p);
-  cudaFree(ctx->d_tok.p); cudaFree(ctx->d_ntok.p);
-  cudaFree(ctx->toon_order.p); cudaFree(ctx->toon_sort.p);
   if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
   cf_run_free(ctx->run);
-  delete ctx;
+  delete ctx;   // frees the DevBuf scratch, on the device set above
 }
 
 const char* cf_last_error(cf_ctx* ctx) { return ctx ? ctx->err.c_str() : "null ctx"; }
@@ -1331,8 +1328,8 @@ int cf_scan_host(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint8_t* stream, ui
   int rc = cf_batch_upload(ctx, b, stream, stream_bytes, offsets, n_units, nullptr);
   if (rc) return rc;
   const size_t bytes = (size_t)n_units * p->W * 8;
-  if ((rc = cf_dev_reserve(ctx, ctx->tmp[6], bytes))) return rc;
-  uint64_t* d_bm = (uint64_t*)ctx->tmp[6].p;
+  if ((rc = cf_dev_reserve(ctx, ctx->bitmaps, bytes))) return rc;
+  uint64_t* d_bm = (uint64_t*)ctx->bitmaps.p;
   if ((rc = cf_scan(ctx, p, b, d_bm, nullptr))) return rc;
   CF_CUDA(ctx, cudaMemcpyAsync(h_bitmaps, d_bm, bytes, cudaMemcpyDeviceToHost, 0));
   CF_CUDA(ctx, cudaStreamSynchronize(0));
@@ -1360,12 +1357,12 @@ int cf_sub_host(cf_ctx* ctx, cf_prog* p, cf_batch* b, const uint32_t* units, uin
   if (out_needed) *out_needed = need;
   if (need > out_cap || (!out_bytes && need)) { ctx->err = "output buffer too small"; return CF_E_CAPACITY; }
   if (need) {
-    if ((rc = cf_dev_reserve(ctx, ctx->tmp[13], ((size_t)n_sel + 1) * 8)) || (rc = cf_dev_reserve(ctx, ctx->tmp[14], need))) return rc;
-    uint64_t* d_ooff = (uint64_t*)ctx->tmp[13].p;
-    uint8_t* d_out = (uint8_t*)ctx->tmp[14].p;
+    if ((rc = cf_dev_reserve(ctx, ctx->sub_out_offsets, ((size_t)n_sel + 1) * 8)) || (rc = cf_dev_reserve(ctx, ctx->sub_out, need))) return rc;
+    uint64_t* d_ooff = (uint64_t*)ctx->sub_out_offsets.p;
+    uint8_t* d_out = (uint8_t*)ctx->sub_out.p;
     CF_CUDA(ctx, cudaMemcpy(d_ooff, out_offsets, ((size_t)n_sel + 1) * 8, cudaMemcpyHostToDevice));
-    sub_compact_kernel<<<n_sel, 256>>>(b->d_buf + cf::FRONT_PAD, b->d_offsets, sub_desc_sel(ctx, n_sel), (const uint8_t*)ctx->tmp[8].p,
-                                       (const uint64_t*)ctx->tmp[12].p, d_ooff, d_out, n_sel);
+    sub_compact_kernel<<<n_sel, 256>>>(b->d_buf + cf::FRONT_PAD, b->d_offsets, sub_desc_sel(ctx, n_sel), (const uint8_t*)ctx->sub_scratch.p,
+                                       (const uint64_t*)ctx->sub_rec.p, d_ooff, d_out, n_sel);
     ctx->launches++;
     CF_CUDA(ctx, cudaGetLastError());
     CF_CUDA(ctx, cudaMemcpy(out_bytes, d_out, need, cudaMemcpyDeviceToHost));

@@ -6,7 +6,6 @@
 #include <string.h>
 
 #include <algorithm>
-#include <type_traits>
 
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
@@ -229,6 +228,14 @@ int cf_stage_reserve(cf_ctx* ctx, size_t need) {
   ctx->h_stage_bytes = c;
   return CF_OK;
 }
+// a device buffer of run r, freed by cf_run_free
+template <class T> static int run_alloc(cf_ctx* ctx, cf_run* r, T** p, size_t bytes) {
+  void* q = nullptr;
+  CF_CUDA(ctx, cudaMalloc(&q, bytes ? bytes : 16));
+  r->allocs.push_back(q);
+  *p = (T*)q;
+  return CF_OK;
+}
 // units per warp for the thread-per-unit JSON kernels: fill the GPU with warps first (about 12 resident
 // warps per SM at their register footprint), only then put several units into one warp
 static uint32_t units_per_warp(const cf_ctx* ctx, uint32_t n) {
@@ -238,6 +245,7 @@ static uint32_t units_per_warp(const cf_ctx* ctx, uint32_t n) {
   return u;
 }
 static uint32_t json_blocks(uint32_t n, uint32_t upw) { return ((n + upw - 1) / upw + 1) / 2; }   // two warps per block
+cudaError_t cf_toon_tp_allow_smem() { return cudaFuncSetAttribute(toon_tp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TP_SMEM); }
 extern "C" {
 int cf_json_index(cf_ctx* ctx, cf_batch* b, uint32_t flags, cf_json_token* d_tokens, uint32_t* d_counts, void* cuda_stream) {
   if (!ctx || !b || !d_tokens || !d_counts) return CF_E_BADARG;
@@ -263,15 +271,6 @@ int cf_json_index_host(cf_ctx* ctx, cf_batch* b, uint32_t flags, const uint8_t* 
   return CF_OK;
 }
 
-// TOON device workspace: token / DOM scratch, and the first pass's unit order with the sort behind it (indices | keys in | keys out |
-// radix-sort temp storage).  The context's for cf_toon and cf_run_batch, a run's own for cf_run_enqueue.
-struct ToonWs {
-  void* scratch;
-  uint64_t scratch_bytes;
-  uint32_t* order;
-  uint8_t* sort;
-  size_t sort_bytes;
-};
 // masking of a batch of nbytes / n units: the parser's nodes (in the TOON scratch, which toon_scratch_need sizes for them), the
 // first pass's arena, and the retry list | node index
 static uint64_t mask_nodes(uint64_t nbytes, uint32_t n) { return nbytes / 2 + 4ull * n + 8; }
@@ -287,27 +286,18 @@ static int toon_sort_temp(cf_ctx* ctx, uint32_t n, cudaStream_t st, size_t* byte
                                                          (uint32_t*)nullptr, (int)n, 0, 8, st));
   return CF_OK;
 }
-static int toon_tp_prepare(cf_ctx* ctx) {
-  static bool smem_set = false;
-  if (!smem_set) {
-    CF_CUDA(ctx, cudaFuncSetAttribute(toon_tp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TP_SMEM));
-    smem_set = true;
-  }
-  return CF_OK;
-}
-
-// does `ws` hold the TOON stage of batch b (token-parallel path)?  Host-only, no launch.
-static int toon_ws_check(cf_ctx* ctx, const cf_batch* b, const ToonWs& ws, cudaStream_t st) {
+// does the run's TOON workspace hold the TOON stage of batch b (token-parallel path)?  Host-only, no launch.
+static int toon_ws_check(cf_ctx* ctx, const cf_batch* b, const cf_run* run, cudaStream_t st) {
   size_t sort_tmp = 0;
   int rc;
   if ((rc = toon_sort_temp(ctx, b->n, st, &sort_tmp))) return rc;
-  if (toon_scratch_need(b->nbytes, b->n) > ws.scratch_bytes || toon_sort_tmp_offset(b->n) + sort_tmp > ws.sort_bytes) { ctx->err = "TOON workspace too small"; return CF_E_CAPACITY; }
+  if (toon_scratch_need(b->nbytes, b->n) > run->toon_scratch_bytes || toon_sort_tmp_offset(b->n) + sort_tmp > run->toon_sort_bytes) { ctx->err = "TOON workspace too small"; return CF_E_CAPACITY; }
   return CF_OK;
 }
 
-// the TOON launches on `st` with a workspace that is already large enough (no allocation, no synchronisation)
+// the TOON launches on `st` with the run's TOON workspace, which is already large enough (no allocation, no synchronisation)
 static int toon_enqueue(cf_ctx* ctx, cf_batch* b, uint32_t flags, uint8_t* d_out, uint32_t* d_out_len, int32_t* d_status, const uint8_t* d_unit_stages,
-                        cudaStream_t st, const ToonWs& ws) {
+                        cudaStream_t st, const cf_run* run) {
   const bool tp = !(flags & (CF_TOON_PARSE_ONLY | CF_TOON_SEQUENTIAL));
   if (!tp && d_unit_stages) { ctx->err = "per-unit stage masks need the token-parallel encoder"; return CF_E_BADARG; }
   // the first pass's unit order: key + stable radix sort over its 8 bits, descending
@@ -315,28 +305,27 @@ static int toon_enqueue(cf_ctx* ctx, cf_batch* b, uint32_t flags, uint8_t* d_out
   size_t sort_tmp = 0;
   int rc;
   if (tp && (rc = toon_sort_temp(ctx, b->n, st, &sort_tmp))) return rc;
-  if (toon_scratch_need(b->nbytes, b->n) > ws.scratch_bytes || (tp && o_tmp + sort_tmp > ws.sort_bytes)) { ctx->err = "TOON workspace too small"; return CF_E_CAPACITY; }
+  if (toon_scratch_need(b->nbytes, b->n) > run->toon_scratch_bytes || (tp && o_tmp + sort_tmp > run->toon_sort_bytes)) { ctx->err = "TOON workspace too small"; return CF_E_CAPACITY; }
   const bool prof = ctx->prof_on && (size_t)ctx->prof_used + 2 <= ctx->prof_ev.size();
   if (prof) cudaEventRecord(ctx->prof_ev[ctx->prof_used], st);
   if (tp) {
-    if ((rc = toon_tp_prepare(ctx))) return rc;
-    uint8_t* srt = ws.sort;
+    uint8_t* srt = run->d_toon_sort;
     toon_order_kernel<<<(b->n + 7) / 8, 256, 0, st>>>(b->d_buf + cf::FRONT_PAD, b->d_offsets, b->n, d_unit_stages, srt + o_kin, (uint32_t*)srt);
     ctx->launches++;
     CF_CUDA(ctx, cudaGetLastError());
-    CF_CUDA(ctx, cub::DeviceRadixSort::SortPairsDescending(srt + o_tmp, sort_tmp, srt + o_kin, srt + o_kout, (const uint32_t*)srt, ws.order, (int)b->n, 0, 8, st));
+    CF_CUDA(ctx, cub::DeviceRadixSort::SortPairsDescending(srt + o_tmp, sort_tmp, srt + o_kin, srt + o_kout, (const uint32_t*)srt, run->d_toon_order, (int)b->n, 0, 8, st));
     ctx->launches++;
     const uint32_t grid = (b->n + TP_WARPS - 1) / TP_WARPS;
-    toon_tp_kernel<<<grid, TP_WARPS * 32, TP_SMEM, st>>>(b->d_buf + cf::FRONT_PAD, b->d_offsets, b->n, (cftp::GTok*)ws.scratch, d_out, d_out_len,
-                                                         d_status, flags, d_unit_stages, ws.order);
+    toon_tp_kernel<<<grid, TP_WARPS * 32, TP_SMEM, st>>>(b->d_buf + cf::FRONT_PAD, b->d_offsets, b->n, (cftp::GTok*)run->d_toon_scratch, d_out, d_out_len,
+                                                         d_status, flags, d_unit_stages, run->d_toon_order);
     ctx->launches++;
     CF_CUDA(ctx, cudaGetLastError());
     // the units the fast path handed over: sequential encoder, one unit per warp (they are few)
-    if (!(flags & CF_TOON_NO_HANDOVER)) cf_launch_toon_seq(json_blocks(b->n, 1), st, b->d_buf + cf::FRONT_PAD, b->d_offsets, b->n, (cfj::JNode*)ws.scratch, d_out, d_out_len, d_status,
+    if (!(flags & CF_TOON_NO_HANDOVER)) cf_launch_toon_seq(json_blocks(b->n, 1), st, b->d_buf + cf::FRONT_PAD, b->d_offsets, b->n, (cfj::JNode*)run->d_toon_scratch, d_out, d_out_len, d_status,
                                                      (flags & 1u) | TOON_ONLY_FALLBACK, 1);
   } else {
     const uint32_t upw = units_per_warp(ctx, b->n);
-    cf_launch_toon_seq(json_blocks(b->n, upw), st, b->d_buf + cf::FRONT_PAD, b->d_offsets, b->n, (cfj::JNode*)ws.scratch, d_out, d_out_len,
+    cf_launch_toon_seq(json_blocks(b->n, upw), st, b->d_buf + cf::FRONT_PAD, b->d_offsets, b->n, (cfj::JNode*)run->d_toon_scratch, d_out, d_out_len,
                                                        d_status, flags & ~TOON_ONLY_FALLBACK, upw);
   }
   if (prof) { cudaEventRecord(ctx->prof_ev[ctx->prof_used + 1], st); ctx->prof_used += 2; }
@@ -345,37 +334,13 @@ static int toon_enqueue(cf_ctx* ctx, cf_batch* b, uint32_t flags, uint8_t* d_out
   return CF_OK;
 }
 
-// the context's TOON workspace (cf_toon, cf_run_batch), grown on demand
-static int toon_ctx_ws(cf_ctx* ctx, const cf_batch* b, uint32_t flags, cudaStream_t st, ToonWs* ws) {
-  const uint64_t need = toon_scratch_need(b->nbytes, b->n);
-  if (need > ctx->toon_scratch_bytes) {
-    CF_CUDA(ctx, cudaStreamSynchronize(st));
-    cudaFree(ctx->d_toon_scratch);
-    ctx->d_toon_scratch = nullptr;
-    ctx->toon_scratch_bytes = 0;
-    CF_CUDA(ctx, cudaMalloc(&ctx->d_toon_scratch, need + need / 4));
-    ctx->toon_scratch_bytes = need + need / 4;
-  }
-  if (!(flags & (CF_TOON_PARSE_ONLY | CF_TOON_SEQUENTIAL))) {
-    size_t sort_tmp = 0;
-    int rc;
-    if ((rc = toon_sort_temp(ctx, b->n, st, &sort_tmp))) return rc;
-    if ((rc = cf_dev_reserve(ctx, ctx->toon_order, (size_t)b->n * 4))) return rc;
-    if ((rc = cf_dev_reserve(ctx, ctx->toon_sort, toon_sort_tmp_offset(b->n) + sort_tmp))) return rc;
-  }
-  *ws = ToonWs{ctx->d_toon_scratch, ctx->toon_scratch_bytes, (uint32_t*)ctx->toon_order.p, (uint8_t*)ctx->toon_sort.p, ctx->toon_sort.cap};
-  return CF_OK;
-}
-static int toon_launch(cf_ctx* ctx, cf_batch* b, uint32_t flags, uint8_t* d_out, uint32_t* d_out_len, int32_t* d_status, const uint8_t* d_unit_stages,
-                       cudaStream_t st) {
-  ToonWs ws;
-  const int rc = toon_ctx_ws(ctx, b, flags, st, &ws);
-  return rc ? rc : toon_enqueue(ctx, b, flags, d_out, d_out_len, d_status, d_unit_stages, st, ws);
-}
+static int ctx_run(cf_ctx* ctx, const cf_batch* b, uint32_t stage_mask, int mask_depth, cudaStream_t st, cf_run** out);
 
 int cf_toon(cf_ctx* ctx, cf_batch* b, uint32_t flags, uint8_t* d_out, uint32_t* d_out_len, int32_t* d_status, void* cuda_stream) {
   if (!ctx || !b || !b->n || !d_out || !d_out_len || !d_status) return CF_E_BADARG;
-  return toon_launch(ctx, b, flags, d_out, d_out_len, d_status, nullptr, (cudaStream_t)cuda_stream);
+  cf_run* run;
+  const int rc = ctx_run(ctx, b, CF_STAGE_TOON, 0, (cudaStream_t)cuda_stream, &run);
+  return rc ? rc : toon_enqueue(ctx, b, flags, d_out, d_out_len, d_status, nullptr, (cudaStream_t)cuda_stream, run);
 }
 
 #ifdef CF_TOON_PHASES
@@ -408,17 +373,14 @@ int cf_toon_host(cf_ctx* ctx, cf_batch* b, uint32_t flags, const uint8_t* stream
   if (!out_stream || !out_len || !status) return CF_E_BADARG;
   int rc = cf_batch_upload(ctx, b, stream, stream_bytes, offsets, n_units, nullptr);
   if (rc) return rc;
-  // device: encode in the input's layout, then gather the converted texts so that only they cross PCIe
-  if ((rc = cf_dev_reserve(ctx, ctx->tmp[0], stream_bytes + 16))) return rc;
-  if ((rc = cf_dev_reserve(ctx, ctx->tmp[1], (size_t)n_units * 4))) return rc;
-  if ((rc = cf_dev_reserve(ctx, ctx->tmp[2], (size_t)n_units * 4))) return rc;
-  if ((rc = cf_dev_reserve(ctx, ctx->tmp[3], ((size_t)n_units + 1) * 8))) return rc;
-  uint8_t* d_out = (uint8_t*)ctx->tmp[0].p;
-  uint32_t* d_len = (uint32_t*)ctx->tmp[1].p;
-  int32_t* d_st = (int32_t*)ctx->tmp[2].p;
-  uint64_t* d_ooff = (uint64_t*)ctx->tmp[3].p;
-  rc = cf_toon(ctx, b, flags, d_out, d_len, d_st, nullptr);
-  if (rc) return rc;
+  // device: encode in the input's layout into the context's run, then gather the converted texts so that only they cross PCIe
+  cf_run* run;
+  if ((rc = ctx_run(ctx, b, CF_STAGE_TOON, 0, nullptr, &run)) || (rc = cf_dev_reserve(ctx, ctx->out_offsets, ((size_t)n_units + 1) * 8))) return rc;
+  uint8_t* d_out = run->d_toon_out;
+  uint32_t* d_len = run->d_toon_ls;
+  int32_t* d_st = (int32_t*)(run->d_toon_ls + n_units);
+  uint64_t* d_ooff = (uint64_t*)ctx->out_offsets.p;
+  if ((rc = toon_enqueue(ctx, b, flags, d_out, d_len, d_st, nullptr, nullptr, run))) return rc;
   CF_CUDA(ctx, cudaMemcpy(out_len, d_len, (size_t)n_units * 4, cudaMemcpyDeviceToHost));
   CF_CUDA(ctx, cudaMemcpy(status, d_st, (size_t)n_units * 4, cudaMemcpyDeviceToHost));
   if (flags & CF_TOON_PARSE_ONLY) return CF_OK;
@@ -427,13 +389,13 @@ int cf_toon_host(cf_ctx* ctx, cf_batch* b, uint32_t flags, const uint8_t* stream
   for (uint32_t i = 0; i < n_units; ++i) { ooff[i] = total; total += out_len[i]; }
   ooff[n_units] = total;
   if (!total) return CF_OK;
-  if ((rc = cf_dev_reserve(ctx, ctx->tmp[4], total))) return rc;
+  if ((rc = cf_dev_reserve(ctx, ctx->gathered, total))) return rc;
   if ((rc = cf_stage_reserve(ctx, total))) return rc;
   CF_CUDA(ctx, cudaMemcpy(d_ooff, ooff.data(), ((size_t)n_units + 1) * 8, cudaMemcpyHostToDevice));
-  compact_kernel<<<n_units, 128>>>(d_out, 1, 0, b->d_offsets, d_len, d_ooff, (uint8_t*)ctx->tmp[4].p, n_units);
+  compact_kernel<<<n_units, 128>>>(d_out, 1, 0, b->d_offsets, d_len, d_ooff, (uint8_t*)ctx->gathered.p, n_units);
   ctx->launches++;
   CF_CUDA(ctx, cudaGetLastError());
-  CF_CUDA(ctx, cudaMemcpy(ctx->h_stage, ctx->tmp[4].p, total, cudaMemcpyDeviceToHost));
+  CF_CUDA(ctx, cudaMemcpy(ctx->h_stage, ctx->gathered.p, total, cudaMemcpyDeviceToHost));
   for (uint32_t i = 0; i < n_units; ++i)
     if (out_len[i]) memcpy(out_stream + offsets[i], (const uint8_t*)ctx->h_stage + ooff[i], out_len[i]);
   return CF_OK;
@@ -455,8 +417,8 @@ int cf_classify_keys_host(cf_ctx* ctx, cf_batch* b, const uint8_t* stream, uint6
   if (!ctx || !b || !sensitive) return CF_E_BADARG;
   int rc = cf_batch_upload(ctx, b, stream, stream_bytes, offsets, n_units, nullptr);
   if (rc) return rc;
-  if ((rc = cf_dev_reserve(ctx, ctx->tmp[6], n_units))) return rc;
-  uint8_t* d = (uint8_t*)ctx->tmp[6].p;
+  if ((rc = cf_dev_reserve(ctx, ctx->bitmaps, n_units))) return rc;
+  uint8_t* d = (uint8_t*)ctx->bitmaps.p;
   cf_launch_classify_keys((n_units + 127) / 128, b->d_buf + cf::FRONT_PAD, b->d_offsets, n_units, d);
   ctx->launches++;
   CF_CUDA(ctx, cudaGetLastError());
@@ -642,7 +604,7 @@ static int run_finish(cf_ctx* ctx, cf_run* run, const uint64_t* h_offsets, uint6
     const uint64_t* rec = nullptr;
     if ((rc = cf_sub_device(ctx, run->prog, b, h_offsets, units.data(), nd, run->st, (uint8_t*)ctx->h_stage, &rec))) return rc;
     CF_CUDA(ctx, cudaMemcpyAsync(run->d_def_rec, rec, (size_t)nd * 16, cudaMemcpyHostToDevice, run->st));
-    if ((rc = run_assemble(ctx, run, run->d_def_rec, (const uint8_t*)ctx->tmp[8].p))) return rc;
+    if ((rc = run_assemble(ctx, run, run->d_def_rec, (const uint8_t*)ctx->sub_scratch.p))) return rc;
     CF_CUDA(ctx, cudaStreamSynchronize(run->st));
     if ((rc = run_d2h(ctx, run, run->h_status, run->d_status, sizeof(RunStatus)))) return rc;
   }
@@ -663,8 +625,27 @@ static int run_grow_arena(cf_ctx* ctx, cf_run* run) {
   return CF_OK;
 }
 
-// own_toon == false: the run gets no TOON workspace of its own; cf_run_batch lends it the context's before each enqueue
-static int run_create(cf_ctx* ctx, uint32_t max_units, uint64_t max_stream_bytes, uint64_t sub_arena_bytes, bool own_toon, cf_run** out) {
+// the run's TOON workspace for its max_units / max_stream_bytes, allocated by the first call: token / DOM scratch (also the mask
+// parser's nodes), the first pass's unit order and the sort behind it (indices | keys in | keys out | radix-sort temp storage), TOON
+// output, and lengths | statuses (of the TOON stage or of the masking's first pass).  The sizes are set once every buffer is there.
+static int run_reserve_toon(cf_ctx* ctx, cf_run* r) {
+  if (r->toon_scratch_bytes) return CF_OK;
+  const uint32_t n = r->max_units;
+  const uint64_t scratch = toon_scratch_need(r->max_bytes, n);
+  size_t sort_tmp = 0;
+  int rc;
+  if ((rc = toon_sort_temp(ctx, n, nullptr, &sort_tmp))) return rc;
+  const size_t sort = toon_sort_tmp_offset(n) + sort_tmp;
+  if ((rc = run_alloc(ctx, r, &r->d_toon_scratch, scratch)) || (rc = run_alloc(ctx, r, &r->d_toon_order, (size_t)n * 4)) ||
+      (rc = run_alloc(ctx, r, &r->d_toon_sort, sort)) || (rc = run_alloc(ctx, r, &r->d_toon_out, r->max_bytes + 16)) ||
+      (rc = run_alloc(ctx, r, &r->d_toon_ls, (size_t)n * 8)))
+    return rc;
+  r->toon_scratch_bytes = scratch;
+  r->toon_sort_bytes = sort;
+  return CF_OK;
+}
+
+static int run_create(cf_ctx* ctx, uint32_t max_units, uint64_t max_stream_bytes, uint64_t sub_arena_bytes, cf_run** out) {
   if (!ctx || !out || !max_units) return CF_E_BADARG;
   *out = nullptr;
   CF_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -676,22 +657,7 @@ static int run_create(cf_ctx* ctx, uint32_t max_units, uint64_t max_stream_bytes
   struct Guard { cf_run*& r; ~Guard() { if (r) cf_run_free(r); } } guard{r};   // every error return frees what was made
   const uint32_t n = max_units;
   int rc;
-  auto dev = [&](auto** p, size_t bytes) -> int {
-    void* q = nullptr;
-    CF_CUDA(ctx, cudaMalloc(&q, bytes ? bytes : 16));
-    r->allocs.push_back(q);
-    *p = reinterpret_cast<std::remove_pointer_t<decltype(p)>>(q);
-    return CF_OK;
-  };
-  if (own_toon) {
-    r->toon_scratch_bytes = toon_scratch_need(max_stream_bytes, n);
-    size_t sort_tmp = 0;
-    if ((rc = toon_sort_temp(ctx, n, nullptr, &sort_tmp))) return rc;
-    r->toon_sort_bytes = toon_sort_tmp_offset(n) + sort_tmp;
-    if ((rc = dev(&r->d_toon_scratch, r->toon_scratch_bytes)) || (rc = dev(&r->d_toon_order, (size_t)n * 4)) || (rc = dev(&r->d_toon_sort, r->toon_sort_bytes)) ||
-        (rc = dev(&r->d_toon_out, max_stream_bytes + 16)) || (rc = dev(&r->d_toon_ls, (size_t)n * 8)))
-      return rc;
-  }
+  auto dev = [&](auto** p, size_t bytes) { return run_alloc(ctx, r, p, bytes); };
   CF_CUDA(ctx, cub::DeviceScan::ExclusiveSum(nullptr, r->scan_tmp_bytes, (const uint64_t*)nullptr, (uint64_t*)nullptr, (int)n + 1));
   if ((rc = dev(&r->d_queue, (size_t)ctx->qcap * 8)) || (rc = dev(&r->d_qstate, 32)) || (rc = dev(&r->d_slot, (size_t)n * 4)) || (rc = dev(&r->d_sel, (size_t)n * 4)) ||
       (rc = dev(&r->d_soff, (size_t)n * 8)) || (rc = dev(&r->d_bound, (size_t)n * 8)) || (rc = dev(&r->d_rec, (size_t)n * 16)) ||
@@ -710,13 +676,17 @@ static int run_create(cf_ctx* ctx, uint32_t max_units, uint64_t max_stream_bytes
   CF_CUDA(ctx, cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
   CF_CUDA(ctx, cudaStreamCreateWithPriority(&r->side, cudaStreamNonBlocking, prio_hi));
   for (cudaEvent_t* e : {&r->ev_scan, &r->ev_sub, &r->ev_done}) CF_CUDA(ctx, cudaEventCreateWithFlags(e, cudaEventDisableTiming));
-  if ((rc = toon_tp_prepare(ctx))) return rc;
   *out = r;
   r = nullptr;
   return CF_OK;
 }
 int cf_run_create(cf_ctx* ctx, uint32_t max_units, uint64_t max_stream_bytes, uint64_t sub_arena_bytes, cf_run** out) {
-  return run_create(ctx, max_units, max_stream_bytes, sub_arena_bytes, true, out);
+  int rc = run_create(ctx, max_units, max_stream_bytes, sub_arena_bytes, out);
+  if (!rc && (rc = run_reserve_toon(ctx, *out))) {
+    cf_run_free(*out);
+    *out = nullptr;
+  }
+  return rc;
 }
 
 void cf_run_free(cf_run* run) {
@@ -754,6 +724,26 @@ int cf_run_set_mask(cf_ctx* ctx, cf_run* run, int max_depth) {
   return CF_OK;
 }
 
+// the context's run, the one cf_toon, cf_toon_host and cf_run_batch use, for batch b and the stages of stage_mask.  When b outgrows
+// it, it is made again for a quarter more (its arena keeps its size) once `st` has drained: work queued there may still use the old
+// one.  TOON and MASK reserve its TOON workspace (the mask parser's nodes are the TOON scratch), MASK its masking workspace, so a
+// SCAN / SUB call allocates neither and a context holds one of each.
+static int ctx_run(cf_ctx* ctx, const cf_batch* b, uint32_t stage_mask, int mask_depth, cudaStream_t st, cf_run** out) {
+  if (!b->n) { ctx->err = "the batch holds no units"; return CF_E_BADARG; }
+  int rc;
+  if (!ctx->run || ctx->run->max_units < b->n || ctx->run->max_bytes < b->nbytes) {
+    const uint64_t arena = ctx->run ? ctx->run->arena_bytes : (1ull << 20);
+    if (ctx->run) CF_CUDA(ctx, cudaStreamSynchronize(st));
+    cf_run_free(ctx->run);
+    ctx->run = nullptr;
+    if ((rc = run_create(ctx, b->n + b->n / 4, b->nbytes + b->nbytes / 4 + 4096, arena, &ctx->run))) return rc;
+  }
+  if ((stage_mask & (CF_STAGE_TOON | CF_STAGE_MASK)) && (rc = run_reserve_toon(ctx, ctx->run))) return rc;
+  if ((stage_mask & CF_STAGE_MASK) && (rc = cf_run_set_mask(ctx, ctx->run, mask_depth))) return rc;
+  *out = ctx->run;
+  return CF_OK;
+}
+
 int cf_run_enqueue(cf_ctx* ctx, cf_prog* prog, cf_batch* b, cf_run* run, uint32_t stage_mask, const uint8_t* d_unit_stages, uint32_t toon_flags,
                    cf_verdict* d_verdicts, uint64_t* d_bitmaps_full, uint64_t* d_out_offsets, uint8_t* d_out, uint64_t out_cap, void* cuda_stream) {
   if (!ctx || !b || !run || run->ctx != ctx || !d_verdicts || !d_out_offsets || (!d_out && out_cap)) return CF_E_BADARG;
@@ -768,10 +758,9 @@ int cf_run_enqueue(cf_ctx* ctx, cf_prog* prog, cf_batch* b, cf_run* run, uint32_
   cudaStream_t st = (cudaStream_t)cuda_stream;
   // every check that can fail comes before the first launch, so that an error return leaves nothing queued
   int rc;
-  const ToonWs ws{run->d_toon_scratch, run->toon_scratch_bytes, run->d_toon_order, run->d_toon_sort, run->toon_sort_bytes};
   if (stage_mask & CF_STAGE_TOON) {
     if (!run->d_toon_scratch || !run->d_toon_out) { ctx->err = "the run has no TOON workspace"; return CF_E_BADARG; }
-    if ((rc = toon_ws_check(ctx, b, ws, st))) return rc;
+    if ((rc = toon_ws_check(ctx, b, run, st))) return rc;
   }
   if ((stage_mask & CF_STAGE_MASK) && (mask_nodes(b->nbytes, n) * sizeof(cfj::JNode) > run->toon_scratch_bytes || !run->d_toon_ls ||
                                        mask_arena_need(b->nbytes, n) > run->mask_arena_bytes || mask_nodes(b->nbytes, n) * 4 > run->mask_idx_bytes)) {
@@ -807,7 +796,7 @@ int cf_run_enqueue(cf_ctx* ctx, cf_prog* prog, cf_batch* b, cf_run* run, uint32_
   }
   if (stage_mask & CF_STAGE_TOON) {
     if ((rc = toon_enqueue(ctx, b, toon_flags & ~(CF_TOON_PARSE_ONLY | CF_TOON_SEQUENTIAL | CF_RUN_OUTPUTS_RESIDENT), run->d_toon_out, run->d_toon_ls,
-                           (int32_t*)(run->d_toon_ls + n), d_unit_stages, st, ws))) return rc;
+                           (int32_t*)(run->d_toon_ls + n), d_unit_stages, st, run))) return rc;
   }
   if (stage_mask & CF_STAGE_MASK) {     // first pass, beside the substitution: every unit into its room in the arena
     const uint32_t upw = units_per_warp(ctx, n);
@@ -860,66 +849,38 @@ int cf_run_batch(cf_ctx* ctx, cf_prog* prog, cf_batch* b, const uint8_t* stream,
   }
   ctx->run_out = nullptr; ctx->run_out_bytes = 0;
   uint64_t total = 0;
-  if (!ctx->run || ctx->run->max_units < n_units || ctx->run->max_bytes < stream_bytes) {     // the context's run, grown with the batches
-    const uint64_t arena = ctx->run ? ctx->run->arena_bytes : (1ull << 20);
-    cf_run_free(ctx->run);
-    ctx->run = nullptr;
-    if ((rc = run_create(ctx, n_units + n_units / 4, stream_bytes + stream_bytes / 4 + 4096, arena, false, &ctx->run))) return rc;
-  }
-  cf_run* run = ctx->run;
-  if (stage_mask & CF_STAGE_TOON) {       // the context's TOON workspace, lent to its run: TOON output in tmp[0], lengths | statuses in tmp[2]
-    ToonWs ws;
-    if ((rc = toon_ctx_ws(ctx, b, 0, 0, &ws)) || (rc = cf_dev_reserve(ctx, ctx->tmp[0], stream_bytes + 16)) ||
-        (rc = cf_dev_reserve(ctx, ctx->tmp[2], (size_t)n_units * 8)))
-      return rc;
-    run->d_toon_scratch = ws.scratch; run->toon_scratch_bytes = ws.scratch_bytes;
-    run->d_toon_order = ws.order; run->d_toon_sort = ws.sort; run->toon_sort_bytes = ws.sort_bytes;
-    run->d_toon_out = (uint8_t*)ctx->tmp[0].p;
-    run->d_toon_ls = (uint32_t*)ctx->tmp[2].p;
-  }
-  if (mask) {     // the context's buffers, lent to its run: parser nodes in the TOON scratch, arena in tmp[0], lengths | statuses in tmp[2],
-                  // retry list | node index in tmp[5]
-    ToonWs ws;
-    const uint64_t idx = mask_nodes(stream_bytes, n_units) * 4;
-    if ((rc = toon_ctx_ws(ctx, b, CF_TOON_SEQUENTIAL, 0, &ws)) || (rc = cf_dev_reserve(ctx, ctx->tmp[0], mask_arena_need(stream_bytes, n_units))) ||
-        (rc = cf_dev_reserve(ctx, ctx->tmp[2], (size_t)n_units * 8)) || (rc = cf_dev_reserve(ctx, ctx->tmp[5], (size_t)n_units * 4 + idx)))
-      return rc;
-    run->d_toon_scratch = ws.scratch; run->toon_scratch_bytes = ws.scratch_bytes;
-    run->d_toon_ls = (uint32_t*)ctx->tmp[2].p;
-    run->d_mask_arena = (uint8_t*)ctx->tmp[0].p; run->mask_arena_bytes = ctx->tmp[0].cap;
-    run->d_mask_retry = (uint32_t*)ctx->tmp[5].p; run->d_mask_idx = run->d_mask_retry + n_units; run->mask_idx_bytes = ctx->tmp[5].cap - (size_t)n_units * 4;
-    run->mask_depth = mask_max_depth;
-  }
+  cf_run* run;
+  if ((rc = ctx_run(ctx, b, stage_mask, mask_max_depth, nullptr, &run))) return rc;
   // pinned staging: unit_stages on the way in; verdicts | out_offsets | bitmaps on the way out
   const size_t o_oo = ((size_t)n_units * sizeof(cf_verdict) + 15) & ~(size_t)15, o_bm = (o_oo + ((size_t)n_units + 1) * 8 + 15) & ~(size_t)15;
   const size_t bm_bytes = (stage_mask & CF_STAGE_SCAN) ? (size_t)n_units * W * 8 : 0;
   if ((rc = cf_stage_reserve(ctx, std::max(o_bm + bm_bytes, (size_t)n_units)))) return rc;
   uint8_t* hs = (uint8_t*)ctx->h_stage;
-  if ((rc = cf_dev_reserve(ctx, ctx->tmp[1], (size_t)n_units * sizeof(cf_verdict))) || (rc = cf_dev_reserve(ctx, ctx->tmp[3], ((size_t)n_units + 1) * 8)) ||
-      (bm_bytes && (rc = cf_dev_reserve(ctx, ctx->tmp[6], bm_bytes))) ||
-      (rc = cf_dev_reserve(ctx, ctx->tmp[4], std::max<uint64_t>(16, keep ? stream_bytes : std::min(out_cap, stream_bytes)))))
+  if ((rc = cf_dev_reserve(ctx, ctx->verdicts, (size_t)n_units * sizeof(cf_verdict))) || (rc = cf_dev_reserve(ctx, ctx->out_offsets, ((size_t)n_units + 1) * 8)) ||
+      (bm_bytes && (rc = cf_dev_reserve(ctx, ctx->bitmaps, bm_bytes))) ||
+      (rc = cf_dev_reserve(ctx, ctx->gathered, std::max<uint64_t>(16, keep ? stream_bytes : std::min(out_cap, stream_bytes)))))
     return rc;
   uint8_t* d_us = nullptr;
   if (unit_stages) {
-    if ((rc = cf_dev_reserve(ctx, ctx->tmp[7], n_units))) return rc;
-    d_us = (uint8_t*)ctx->tmp[7].p;
+    if ((rc = cf_dev_reserve(ctx, ctx->unit_stages, n_units))) return rc;
+    d_us = (uint8_t*)ctx->unit_stages.p;
     memcpy(hs, unit_stages, n_units);
     CF_CUDA(ctx, cudaMemcpyAsync(d_us, hs, n_units, cudaMemcpyHostToDevice, 0));
   }
-  cf_verdict* d_v = (cf_verdict*)ctx->tmp[1].p;
-  uint64_t* d_oo = (uint64_t*)ctx->tmp[3].p;
+  cf_verdict* d_v = (cf_verdict*)ctx->verdicts.p;
+  uint64_t* d_oo = (uint64_t*)ctx->out_offsets.p;
   // the device buffer takes what the caller can take (all of it when the texts stay resident); a shortfall of the device buffer alone
   // is made up below by growing it and gathering again
-  uint8_t* d_out = (uint8_t*)ctx->tmp[4].p;
-  const uint64_t dcap = keep ? ctx->tmp[4].cap : (out_bytes ? std::min<uint64_t>(ctx->tmp[4].cap, out_cap) : 0);
+  uint8_t* d_out = (uint8_t*)ctx->gathered.p;
+  const uint64_t dcap = keep ? ctx->gathered.cap : (out_bytes ? std::min<uint64_t>(ctx->gathered.cap, out_cap) : 0);
   nvtxRangePushA("cf_run_batch:kernels");
-  rc = cf_run_enqueue(ctx, prog, b, run, stage_mask, d_us, toon_flags, d_v, bm_bytes ? (uint64_t*)ctx->tmp[6].p : nullptr, d_oo, d_out, dcap, nullptr);
+  rc = cf_run_enqueue(ctx, prog, b, run, stage_mask, d_us, toon_flags, d_v, bm_bytes ? (uint64_t*)ctx->bitmaps.p : nullptr, d_oo, d_out, dcap, nullptr);
   bool out_short = false;
   if (!rc) rc = run_finish(ctx, run, offsets, &total, &out_short);
   nvtxRangePop();
   if (out_short && (keep || (out_bytes && total <= out_cap))) {
-    if ((rc = cf_dev_reserve(ctx, ctx->tmp[4], total))) return rc;
-    run->d_out = (uint8_t*)ctx->tmp[4].p;
+    if ((rc = cf_dev_reserve(ctx, ctx->gathered, total))) return rc;
+    run->d_out = (uint8_t*)ctx->gathered.p;
     run->out_cap = total;
     if ((rc = run_gather(ctx, run))) return rc;
     CF_CUDA(ctx, cudaStreamSynchronize(0));
@@ -933,9 +894,9 @@ int cf_run_batch(cf_ctx* ctx, cf_prog* prog, cf_batch* b, const uint8_t* stream,
   hs = (uint8_t*)ctx->h_stage;
   CF_CUDA(ctx, cudaMemcpyAsync(hs, d_v, (size_t)n_units * sizeof(cf_verdict), cudaMemcpyDeviceToHost, 0));
   CF_CUDA(ctx, cudaMemcpyAsync(hs + o_oo, d_oo, ((size_t)n_units + 1) * 8, cudaMemcpyDeviceToHost, 0));
-  if (bitmaps_full && bm_bytes) CF_CUDA(ctx, cudaMemcpyAsync(hs + o_bm, ctx->tmp[6].p, bm_bytes, cudaMemcpyDeviceToHost, 0));
+  if (bitmaps_full && bm_bytes) CF_CUDA(ctx, cudaMemcpyAsync(hs + o_bm, ctx->bitmaps.p, bm_bytes, cudaMemcpyDeviceToHost, 0));
   const bool fits = keep || (total <= out_cap && (out_bytes || !total));
-  if (fits && !keep && total) CF_CUDA(ctx, cudaMemcpyAsync(out_bytes, ctx->tmp[4].p, total, cudaMemcpyDeviceToHost, 0));
+  if (fits && !keep && total) CF_CUDA(ctx, cudaMemcpyAsync(out_bytes, ctx->gathered.p, total, cudaMemcpyDeviceToHost, 0));
   CF_CUDA(ctx, cudaStreamSynchronize(0));
   memcpy(verdicts, hs, (size_t)n_units * sizeof(cf_verdict));
   memcpy(out_offsets, hs + o_oo, ((size_t)n_units + 1) * 8);
@@ -943,7 +904,7 @@ int cf_run_batch(cf_ctx* ctx, cf_prog* prog, cf_batch* b, const uint8_t* stream,
   if (out_needed) *out_needed = total;
   if (!fits) { ctx->err = "output buffer too small"; return CF_E_CAPACITY; }
   if (keep) {
-    ctx->run_out = total ? (const uint8_t*)ctx->tmp[4].p : nullptr;
+    ctx->run_out = total ? (const uint8_t*)ctx->gathered.p : nullptr;
     ctx->run_out_bytes = total;
   }
   return CF_OK;
