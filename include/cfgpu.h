@@ -201,12 +201,15 @@ int cf_json_index_host(cf_ctx* ctx, cf_batch* b, uint32_t flags, const uint8_t* 
 #define CF_TOON_PARSE_ONLY 4u    /* flags, diagnostic: only parse; status = 0 ok / 1 invalid JSON / 2 beyond limits,
                                   * out_len = DOM node count (used by tools/toon_prof.py to time the parser alone) */
 #define CF_TOON_SEQUENTIAL 8u    /* flags, diagnostic: skip the token-parallel kernel (csrc/json_tp.h), run every unit through the
-                                  * sequential per-thread encoder (the one that otherwise only takes the units the fast path hands over) */
+                                  * sequential per-thread encoder (the one that otherwise only takes the units the fast path hands over).
+                                  * cf_run_batch and cf_run_enqueue accept it in toon_flags when unit_stages is NULL (CF_E_BADARG otherwise) */
 #define CF_TOON_NO_HANDOVER 16u  /* flags, diagnostic: leave the units the token-parallel kernel does not cover at status 7 with the
                                   * reason (json_tp.h FB_*) in out_len instead of re-doing them with the sequential encoder */
 /* device-resident (batch already uploaded); d_out has room for the batch's stream bytes */
 int cf_toon(cf_ctx* ctx, cf_batch* b, uint32_t flags, uint8_t* d_out, uint32_t* d_out_len, int32_t* d_status, void* cuda_stream);
-/* host buffers: upload + encode + download, synchronous */
+/* host buffers: upload + encode + download, synchronous.  cf_run_batch(CF_STAGE_TOON) into out_stream (stream_bytes bytes), then each
+ * text moved from its packed place to its unit's offset; out_stream's other bytes are unspecified.  The texts are copied from the device
+ * straight into out_stream, so page-locked memory (cf_host_alloc) keeps that copy at the PCIe rate.  CF_TOON_PARSE_ONLY writes no text. */
 int cf_toon_host(cf_ctx* ctx, cf_batch* b, uint32_t flags, const uint8_t* stream, uint64_t stream_bytes, const uint64_t* offsets,
                  uint32_t n_units, uint8_t* out_stream, uint32_t* out_len, int32_t* status);
 

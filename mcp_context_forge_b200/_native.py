@@ -14,6 +14,7 @@ CF_E_CUDA, CF_E_BADARG, CF_E_UNSUPPORTED, CF_E_TOO_LARGE, CF_E_CAPACITY, CF_E_NO
 CF_PAT_SEARCH, CF_PAT_ORDERED = 0, 1
 CF_STAGE_SCAN, CF_STAGE_SUB, CF_STAGE_MASK, CF_STAGE_TOON = 1, 2, 4, 8
 CF_RUN_OUTPUTS_RESIDENT = 32
+CF_TOON_REPORT_ERRORS, CF_TOON_PARSE_ONLY, CF_TOON_SEQUENTIAL, CF_TOON_NO_HANDOVER = 1, 4, 8, 16
 CF_V_REWRITTEN, CF_V_TOON, CF_V_MASKED, CF_V_RESUBMIT = 1, 2, 4, 8
 ERR_NAMES = {-1: "CF_E_CUDA", -2: "CF_E_BADARG", -3: "CF_E_UNSUPPORTED", -4: "CF_E_TOO_LARGE", -5: "CF_E_CAPACITY", -6: "CF_E_NOGPU", -7: "CF_E_NOMEM"}
 

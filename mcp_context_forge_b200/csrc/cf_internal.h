@@ -50,8 +50,8 @@ struct cf_ctx {
   DevBuf sub_scratch, sub_desc, sub_rec, sub_pike;
   DevBuf sub_out_offsets, sub_out;  // cf_sub_host's gather of the rewritten texts
   DevBuf verdicts, unit_stages;     // cf_run_batch with host buffers: verdict records, per-unit stage masks on the way in
-  // the gather of cf_run_batch and of cf_toon_host: out offsets and the gathered texts.  Shared, as neither call's texts outlive it,
-  // except `gathered` after a CF_RUN_OUTPUTS_RESIDENT cf_run_batch: cf_run_batch_device_output hands it out until either call runs again
+  // the gather of cf_run_batch (and so of cf_toon_host and cf_mask_host): out offsets and the gathered texts, which no call outlives,
+  // except `gathered` after a CF_RUN_OUTPUTS_RESIDENT call: cf_run_batch_device_output hands it out until cf_run_batch runs again
   DevBuf out_offsets, gathered;
   DevBuf bitmaps;                   // pattern bitmaps of cf_scan_host and cf_run_batch, or cf_classify_keys_host's flags
   DevBuf d_tok, d_ntok;             // structural index of the current batch (json_index_kernel)

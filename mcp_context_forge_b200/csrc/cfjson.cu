@@ -197,19 +197,6 @@ __global__ void __launch_bounds__(256) toon_order_kernel(const uint8_t* __restri
   }
 }
 
-// gather per-unit results (unit u at src + mul*offsets[u] + add*u, out_len[u] bytes) into one contiguous buffer
-__global__ void compact_kernel(const uint8_t* __restrict__ src, uint32_t mul, uint32_t add, const uint64_t* __restrict__ offsets,
-                               const uint32_t* __restrict__ out_len, const uint64_t* __restrict__ out_off, uint8_t* __restrict__ out,
-                               uint32_t n_units) {
-  const uint32_t u = blockIdx.x;
-  if (u >= n_units) return;
-  const uint8_t* s = src + (uint64_t)mul * offsets[u] + (uint64_t)add * u;
-  uint8_t* dst = out + out_off[u];
-  for (uint32_t i = threadIdx.x; i < out_len[u]; i += blockDim.x) dst[i] = s[i];
-}
-
-
-
 int cf_dev_reserve(cf_ctx* ctx, cf_ctx::DevBuf& b, size_t need) {
   if (need <= b.cap) return CF_OK;
   cudaFree(b.p);
@@ -299,7 +286,6 @@ static int toon_ws_check(cf_ctx* ctx, const cf_batch* b, const cf_run* run, cuda
 static int toon_enqueue(cf_ctx* ctx, cf_batch* b, uint32_t flags, uint8_t* d_out, uint32_t* d_out_len, int32_t* d_status, const uint8_t* d_unit_stages,
                         cudaStream_t st, const cf_run* run) {
   const bool tp = !(flags & (CF_TOON_PARSE_ONLY | CF_TOON_SEQUENTIAL));
-  if (!tp && d_unit_stages) { ctx->err = "per-unit stage masks need the token-parallel encoder"; return CF_E_BADARG; }
   // the first pass's unit order: key + stable radix sort over its 8 bits, descending
   const size_t o_kin = (size_t)b->n * 4, o_kout = o_kin + b->n, o_tmp = toon_sort_tmp_offset(b->n);
   size_t sort_tmp = 0;
@@ -371,33 +357,28 @@ void cf_toon_tp_config(uint32_t* warps_per_cta, uint32_t* ctas_per_sm, uint32_t*
 int cf_toon_host(cf_ctx* ctx, cf_batch* b, uint32_t flags, const uint8_t* stream, uint64_t stream_bytes, const uint64_t* offsets,
                  uint32_t n_units, uint8_t* out_stream, uint32_t* out_len, int32_t* status) {
   if (!out_stream || !out_len || !status) return CF_E_BADARG;
-  int rc = cf_batch_upload(ctx, b, stream, stream_bytes, offsets, n_units, nullptr);
-  if (rc) return rc;
-  // device: encode in the input's layout into the context's run, then gather the converted texts so that only they cross PCIe
-  cf_run* run;
-  if ((rc = ctx_run(ctx, b, CF_STAGE_TOON, 0, nullptr, &run)) || (rc = cf_dev_reserve(ctx, ctx->out_offsets, ((size_t)n_units + 1) * 8))) return rc;
-  uint8_t* d_out = run->d_toon_out;
-  uint32_t* d_len = run->d_toon_ls;
-  int32_t* d_st = (int32_t*)(run->d_toon_ls + n_units);
-  uint64_t* d_ooff = (uint64_t*)ctx->out_offsets.p;
-  if ((rc = toon_enqueue(ctx, b, flags, d_out, d_len, d_st, nullptr, nullptr, run))) return rc;
-  CF_CUDA(ctx, cudaMemcpy(out_len, d_len, (size_t)n_units * 4, cudaMemcpyDeviceToHost));
-  CF_CUDA(ctx, cudaMemcpy(status, d_st, (size_t)n_units * 4, cudaMemcpyDeviceToHost));
-  if (flags & CF_TOON_PARSE_ONLY) return CF_OK;
-  std::vector<uint64_t> ooff((size_t)n_units + 1);
-  uint64_t total = 0;
-  for (uint32_t i = 0; i < n_units; ++i) { ooff[i] = total; total += out_len[i]; }
-  ooff[n_units] = total;
-  if (!total) return CF_OK;
-  if ((rc = cf_dev_reserve(ctx, ctx->gathered, total))) return rc;
-  if ((rc = cf_stage_reserve(ctx, total))) return rc;
-  CF_CUDA(ctx, cudaMemcpy(d_ooff, ooff.data(), ((size_t)n_units + 1) * 8, cudaMemcpyHostToDevice));
-  compact_kernel<<<n_units, 128>>>(d_out, 1, 0, b->d_offsets, d_len, d_ooff, (uint8_t*)ctx->gathered.p, n_units);
-  ctx->launches++;
-  CF_CUDA(ctx, cudaGetLastError());
-  CF_CUDA(ctx, cudaMemcpy(ctx->h_stage, ctx->gathered.p, total, cudaMemcpyDeviceToHost));
-  for (uint32_t i = 0; i < n_units; ++i)
-    if (out_len[i]) memcpy(out_stream + offsets[i], (const uint8_t*)ctx->h_stage + ooff[i], out_len[i]);
+  int rc;
+  if (flags & CF_TOON_PARSE_ONLY) {     // out_len is a node count: no texts to gather
+    cf_run* run;
+    if ((rc = cf_batch_upload(ctx, b, stream, stream_bytes, offsets, n_units, nullptr)) || (rc = ctx_run(ctx, b, CF_STAGE_TOON, 0, nullptr, &run)) ||
+        (rc = toon_enqueue(ctx, b, flags, run->d_toon_out, run->d_toon_ls, (int32_t*)(run->d_toon_ls + n_units), nullptr, nullptr, run)))
+      return rc;
+  } else {
+    // the fused chain's TOON stage packs the converted texts into out_stream; every one is shorter than its unit, so they fit
+    std::vector<cf_verdict> v(n_units);
+    std::vector<uint64_t> packed((size_t)n_units + 1);
+    if ((rc = cf_run_batch(ctx, nullptr, b, stream, stream_bytes, offsets, n_units, CF_STAGE_TOON, nullptr,
+                           flags & (CF_TOON_REPORT_ERRORS | CF_TOON_SEQUENTIAL | CF_TOON_NO_HANDOVER), 0, v.data(), nullptr, out_stream, stream_bytes,
+                           packed.data(), nullptr)))
+      return rc;
+    // each text from its packed place to its unit's, last unit first: packed[i] <= offsets[i], so no move overwrites a text still to move
+    for (uint32_t i = n_units; i-- > 0;)
+      if (packed[i + 1] > packed[i]) memmove(out_stream + offsets[i], out_stream + packed[i], packed[i + 1] - packed[i]);
+  }
+  // the encoder's own lengths and statuses: under CF_TOON_NO_HANDOVER a handed-over unit's out_len is its reason, which verdicts drop
+  const uint32_t* d_ls = ctx->run->d_toon_ls;
+  CF_CUDA(ctx, cudaMemcpy(out_len, d_ls, (size_t)n_units * 4, cudaMemcpyDeviceToHost));
+  CF_CUDA(ctx, cudaMemcpy(status, d_ls + n_units, (size_t)n_units * 4, cudaMemcpyDeviceToHost));
   return CF_OK;
 }
 
@@ -760,6 +741,7 @@ int cf_run_enqueue(cf_ctx* ctx, cf_prog* prog, cf_batch* b, cf_run* run, uint32_
   int rc;
   if (stage_mask & CF_STAGE_TOON) {
     if (!run->d_toon_scratch || !run->d_toon_out) { ctx->err = "the run has no TOON workspace"; return CF_E_BADARG; }
+    if ((toon_flags & CF_TOON_SEQUENTIAL) && d_unit_stages) { ctx->err = "per-unit stage masks need the token-parallel encoder"; return CF_E_BADARG; }
     if ((rc = toon_ws_check(ctx, b, run, st))) return rc;
   }
   if ((stage_mask & CF_STAGE_MASK) && (mask_nodes(b->nbytes, n) * sizeof(cfj::JNode) > run->toon_scratch_bytes || !run->d_toon_ls ||
@@ -795,7 +777,7 @@ int cf_run_enqueue(cf_ctx* ctx, cf_prog* prog, cf_batch* b, cf_run* run, uint32_
     CF_CUDA(ctx, cudaEventRecord(run->ev_sub, run->side));
   }
   if (stage_mask & CF_STAGE_TOON) {
-    if ((rc = toon_enqueue(ctx, b, toon_flags & ~(CF_TOON_PARSE_ONLY | CF_TOON_SEQUENTIAL | CF_RUN_OUTPUTS_RESIDENT), run->d_toon_out, run->d_toon_ls,
+    if ((rc = toon_enqueue(ctx, b, toon_flags & ~(CF_TOON_PARSE_ONLY | CF_RUN_OUTPUTS_RESIDENT), run->d_toon_out, run->d_toon_ls,
                            (int32_t*)(run->d_toon_ls + n), d_unit_stages, st, run))) return rc;
   }
   if (stage_mask & CF_STAGE_MASK) {     // first pass, beside the substitution: every unit into its room in the arena

@@ -472,23 +472,35 @@ def device_output(ctx: Context) -> np.ndarray:
 def toon_host(batch: Batch, stream, offsets: np.ndarray, report_errors: bool = True):
     """cf_toon_host: every unit is one JSON text.  Returns (status int32[n], toon texts as bytes or
     None per unit)."""
+    status, texts, _ = toon_host_flags(batch, stream, offsets, N.CF_TOON_REPORT_ERRORS if report_errors else 0)
+    return status, texts
+
+
+def toon_host_flags(batch: Batch, stream, offsets: np.ndarray, flags: int):
+    """cf_toon_host with any CF_TOON_* flags.  Returns (status int32[n], toon texts as bytes or None per unit, out_len uint32[n]: the
+    text's length, the hand-over reason under CF_TOON_NO_HANDOVER, the node count under CF_TOON_PARSE_ONLY, which returns no texts)."""
     ctx = batch.ctx
     n = len(offsets) - 1
     nbytes = int(offsets[-1])
-    out = np.empty(max(nbytes, 1), dtype=np.uint8)
+    # the texts land in the Batch's page-locked output buffer (run_batch's), so that their D2H runs at the PCIe rate
+    pin = getattr(batch, "_out_pin", None)
+    if pin is None or pin.nbytes < nbytes:
+        batch._out_pin = None                              # free before growing
+        pin = batch._out_pin = PinnedBuffer(ctx, max(nbytes, 1 << 12))
+    out = pin.array
     out_len = np.empty(n, dtype=np.uint32)
     status = np.empty(n, dtype=np.int32)
     sp = stream.ctypes.data if isinstance(stream, np.ndarray) else ctypes.cast(ctypes.c_char_p(stream), c_void_p)
     with ctx.lock:
-        ctx.check(ctx.lib.cf_toon_host(ctx.h, batch.h, 1 if report_errors else 0, sp, nbytes, offsets.ctypes.data, n, out.ctypes.data, out_len.ctypes.data, status.ctypes.data), "cf_toon_host")
+        ctx.check(ctx.lib.cf_toon_host(ctx.h, batch.h, flags, sp, nbytes, offsets.ctypes.data, n, out.ctypes.data, out_len.ctypes.data, status.ctypes.data), "cf_toon_host")
     texts: List[Optional[bytes]] = []
     for i in range(n):
-        if status[i] == TOON_CONVERTED:
+        if status[i] == TOON_CONVERTED and not flags & N.CF_TOON_PARSE_ONLY:
             o = int(offsets[i])
             texts.append(out[o:o + int(out_len[i])].tobytes())
         else:
             texts.append(None)
-    return status, texts
+    return status, texts, out_len
 
 
 def json_index_host(batch: Batch, stream, offsets: np.ndarray, classify: bool = False):

@@ -84,16 +84,6 @@ def check_chain(units, v, out, oo, full, toon):
     assert max(int(oo[i + 1] - oo[i]) for i in range(len(units))) > 1 << 16
 
 
-def toon_host(ctx, batch, stream, offs, flags):
-    n = len(offs) - 1
-    out = np.zeros(len(stream), dtype=np.uint8)
-    out_len = np.zeros(n, dtype=np.uint32)
-    status = np.full(n, -1, dtype=np.int32)
-    ctx.check(ctx.lib.cf_toon_host(ctx.h, batch.h, flags, ctypes.cast(ctypes.c_char_p(stream), ctypes.c_void_p), len(stream), offs.ctypes.data, n,
-                                   out.ctypes.data, out_len.ctypes.data, status.ctypes.data), "cf_toon_host")
-    return status, [out[int(offs[i]):int(offs[i]) + int(out_len[i])].tobytes().decode() if status[i] == engine.TOON_CONVERTED else None for i in range(n)]
-
-
 def is_json(u):
     try:
         json.loads(u)
@@ -148,9 +138,9 @@ def run_sequence(ctx, prog, units):
     assert resident_output(ctx) == resident and read_device(ctx, *resident) == texts
     # cf_toon_host on every route
     for flags in (REPORT_ERRORS, SEQUENTIAL | REPORT_ERRORS):
-        _, got = toon_host(ctx, batch, stream, offs, flags)
-        assert got == exp_toon, flags
-    status, _ = toon_host(ctx, batch, stream, offs, PARSE_ONLY)
+        _, got, _ = engine.toon_host_flags(batch, stream, offs, flags)
+        assert [None if t is None else t.decode() for t in got] == exp_toon, flags
+    status, _, _ = engine.toon_host_flags(batch, stream, offs, PARSE_ONLY)
     assert [int(x) for x in status] == [0 if is_json(u) else 1 for u in units]
     # SCAN|MASK at two depths: the masking workspace is reused, and at depth 2 the last two bodies outgrow their first room
     for md in (10, 2):

@@ -8,11 +8,9 @@ UNSUPPORTED (6) instead; masking parses serde_json's 127 levels, so it holds the
 
 A second corpus reaches every reason (json_tp.h FB_*) for which the token-parallel kernel hands a unit to the sequential
 encoder: with CF_TOON_NO_HANDOVER the reason is reported, on the default path the unit gets the oracle's answer."""
-import ctypes
 import random
 import struct
 
-import numpy as np
 import pytest
 
 from mcp_context_forge_b200 import engine
@@ -179,16 +177,8 @@ def mask_oracle(b, md):
 def toon_call(ctx, units, flags):
     """cf_toon_host with explicit flags: (status int32[n], out_len uint32[n], texts)."""
     stream, offs = engine.pack_units(units)
-    n = len(units)
-    batch = engine.Batch(ctx, len(stream), n)
-    out = np.empty(max(len(stream), 1), dtype=np.uint8)
-    out_len = np.empty(n, dtype=np.uint32)
-    status = np.empty(n, dtype=np.int32)
-    with ctx.lock:
-        ctx.check(ctx.lib.cf_toon_host(ctx.h, batch.h, flags, ctypes.cast(ctypes.c_char_p(stream), ctypes.c_void_p), len(stream), offs.ctypes.data, n,
-                                       out.ctypes.data, out_len.ctypes.data, status.ctypes.data), "cf_toon_host")
-    texts = [out[int(offs[i]):int(offs[i]) + int(out_len[i])].tobytes().decode("utf-8") if status[i] == engine.TOON_CONVERTED else None for i in range(n)]
-    return status, out_len, texts
+    status, texts, out_len = engine.toon_host_flags(engine.Batch(ctx, len(stream), len(units)), stream, offs, flags)
+    return status, out_len, [None if t is None else t.decode("utf-8") for t in texts]
 
 
 def check_toon(units, flags):

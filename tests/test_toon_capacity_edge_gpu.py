@@ -8,7 +8,6 @@ The edge documents sit among ordinary neighbours in launches of about 200, 6 000
 warps walk 1, 4 and 32 units each (cfjson.cu units_per_warp on an H100) and the token-parallel kernel meets the boundary at many
 unit alignments."""
 import asyncio
-import ctypes
 import os
 import random
 import tempfile
@@ -88,16 +87,8 @@ def launches(n_docs):
 
 # ---------------------------------------------------------------------------------------------------------------------- routes
 def toon_host(ctx, stream, offs, n, flags):
-    out = np.empty(max(len(stream), 1), dtype=np.uint8)
-    out_len = np.empty(n, dtype=np.uint32)
-    status = np.empty(n, dtype=np.int32)
-    batch = engine.Batch(ctx, len(stream), n)
-    with ctx.lock:
-        ctx.check(ctx.lib.cf_toon_host(ctx.h, batch.h, flags, ctypes.cast(ctypes.c_char_p(stream), ctypes.c_void_p),
-                                       len(stream), offs.ctypes.data, n, out.ctypes.data, out_len.ctypes.data, status.ctypes.data), "cf_toon_host")
-    raw = out.tobytes()
-    res = [(int(s), raw[int(offs[i]):int(offs[i]) + int(out_len[i])].decode("utf-8") if s == 0 else None) for i, s in enumerate(status)]
-    return res, out_len.tolist()
+    status, texts, out_len = engine.toon_host_flags(engine.Batch(ctx, len(stream), n), stream, offs, flags)
+    return [(int(s), None if t is None else t.decode("utf-8")) for s, t in zip(status, texts)], out_len.tolist()
 
 
 def from_verdicts(v, raw, oo):

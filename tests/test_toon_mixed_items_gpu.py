@@ -1,12 +1,10 @@
 """Mixed list-item arrays (see test_toon_mixed_items_cpu.py) through the whole TOON stage on the GPU: the first token-parallel pass,
 the resolving pass for the units it hands over as mixed, the sequential encoder for the rest.  Every result equals the oracle, as do
 the results of bench.py's payload mix."""
-import ctypes
 import json
 import os
 import sys
 
-import numpy as np
 import pytest
 
 from mcp_context_forge_b200 import engine
@@ -24,14 +22,8 @@ def toon(texts, flags):
     ctx = engine.Context.get()
     enc = [engine.encode_unit(t) for t in texts]
     stream, offs = engine.pack_units(enc)
-    batch = engine.Batch(ctx, len(stream), len(enc))
-    n = len(enc)
-    out = np.zeros(max(len(stream), 1), dtype=np.uint8)
-    out_len = np.zeros(n, dtype=np.uint32)
-    status = np.zeros(n, dtype=np.int32)
-    ctx.check(ctx.lib.cf_toon_host(ctx.h, batch.h, flags, ctypes.cast(ctypes.c_char_p(stream), ctypes.c_void_p), len(stream), offs.ctypes.data, n,
-                                   out.ctypes.data, out_len.ctypes.data, status.ctypes.data), "cf_toon_host")
-    return [(int(status[i]), out[int(offs[i]):int(offs[i]) + int(out_len[i])].tobytes().decode() if status[i] == 0 else None) for i in range(n)]
+    status, got, _ = engine.toon_host_flags(engine.Batch(ctx, len(stream), len(enc)), stream, offs, flags)
+    return [(int(s), None if g is None else g.decode()) for s, g in zip(status, got)]
 
 
 @pytest.mark.parametrize("flags", [0, REPORT_ERRORS])

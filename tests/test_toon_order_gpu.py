@@ -176,3 +176,18 @@ def test_per_unit_stages(prog):
                 assert r == all_toon[i], i
             else:
                 assert r[2] == engine.TOON_SKIPPED and not r[0] & N.CF_V_TOON and r[1] == 0, i
+
+
+def test_sequential_encoder_refuses_per_unit_stages(prog):
+    """CF_TOON_SEQUENTIAL reaches the run, whose sequential encoder takes no per-unit stage masks: cf_run_batch refuses the pair
+    before anything is queued, and the same batch then runs as before."""
+    units = corpus()
+    stream, offs = engine.pack_units([engine.encode_unit(u) for u in units])
+    batch = engine.Batch(engine.Context.get(), len(stream), len(units))
+    stages = np.full(len(units), N.CF_STAGE_SCAN | N.CF_STAGE_TOON, dtype=np.uint8)
+    with pytest.raises(N.CfError) as err:
+        engine.run_batch(prog, batch, stream, offs, N.CF_STAGE_SCAN | N.CF_STAGE_TOON, unit_stages=stages, toon_flags=N.CF_TOON_SEQUENTIAL)
+    assert err.value.code == N.CF_E_BADARG
+    v, _, _, _ = engine.run_batch(prog, batch, stream, offs, N.CF_STAGE_SCAN | N.CF_STAGE_TOON,
+                                  toon_flags=N.CF_TOON_SEQUENTIAL | N.CF_TOON_REPORT_ERRORS)
+    assert [int(a) for a in v["aux"]] == [s for s, _ in toon_host(units)]

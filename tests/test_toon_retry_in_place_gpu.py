@@ -3,7 +3,6 @@ family, bench.py's payload mix and a unit whose retry runs out of key-stack room
 and sorted, through cf_toon_host and through cf_run_batch with host buffers and resident.  No unit is left at status 7 and every text
 equals the oracle's; with CF_TOON_NO_HANDOVER the kernel makes the first attempt only, so a mixed unit reports FB_MIXED_ITEM as the
 emulated first attempt does."""
-import ctypes
 import json
 import os
 import sys
@@ -44,14 +43,8 @@ def toon_host(texts, flags):
     """cf_toon_host: [(status, reason or TOON text)] per unit."""
     ctx = engine.Context.get()
     stream, offs = engine.pack_units([engine.encode_unit(t) for t in texts])
-    n = len(texts)
-    batch = engine.Batch(ctx, len(stream), n)
-    out = np.zeros(max(len(stream), 1), dtype=np.uint8)
-    out_len = np.zeros(n, dtype=np.uint32)
-    status = np.zeros(n, dtype=np.int32)
-    ctx.check(ctx.lib.cf_toon_host(ctx.h, batch.h, flags, ctypes.cast(ctypes.c_char_p(stream), ctypes.c_void_p), len(stream), offs.ctypes.data, n,
-                                   out.ctypes.data, out_len.ctypes.data, status.ctypes.data), "cf_toon_host")
-    return [(int(status[i]), out[int(offs[i]):int(offs[i]) + int(out_len[i])].tobytes().decode() if status[i] == 0 else int(out_len[i])) for i in range(n)]
+    status, got, out_len = engine.toon_host_flags(engine.Batch(ctx, len(stream), len(texts)), stream, offs, flags)
+    return [(int(s), int(k) if g is None else g.decode()) for s, g, k in zip(status, got, out_len)]
 
 
 @pytest.fixture(scope="module")

@@ -1,9 +1,6 @@
 """The tokenizer's lane- and step-edge cases of tests/test_toon_tokenize_steps_cpu.py on the GPU: toon_tp_kernel (its step-wise UTF-8
 check, its number classification) against the sequential encoder on the same device, through cf_toon_host.
 Units are packed one after the other, so their alignments vary."""
-import ctypes
-
-import numpy as np
 import pytest
 
 import test_toon_tokenize_steps_cpu as cases
@@ -16,14 +13,8 @@ SEQ, NOFB = 8, 16
 def toon(texts, flags):
     ctx = engine.Context.get()
     stream, offs = engine.pack_units(texts)
-    batch = engine.Batch(ctx, len(stream), len(texts))
-    n = len(texts)
-    out = np.zeros(max(len(stream), 1), dtype=np.uint8)
-    out_len = np.zeros(n, dtype=np.uint32)
-    status = np.zeros(n, dtype=np.int32)
-    ctx.check(ctx.lib.cf_toon_host(ctx.h, batch.h, flags, ctypes.cast(ctypes.c_char_p(stream), ctypes.c_void_p), len(stream), offs.ctypes.data, n,
-                                   out.ctypes.data, out_len.ctypes.data, status.ctypes.data), "cf_toon_host")
-    return [(int(status[i]), out[int(offs[i]):int(offs[i]) + int(out_len[i])].tobytes() if status[i] == 0 else None) for i in range(n)], status, out_len
+    status, got, out_len = engine.toon_host_flags(engine.Batch(ctx, len(stream), len(texts)), stream, offs, flags)
+    return [(int(s), g) for s, g in zip(status, got)], status, out_len
 
 
 def _texts():

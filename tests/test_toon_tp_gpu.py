@@ -1,13 +1,11 @@
 """GPU parity of the token-parallel TOON kernel (toon_tp_kernel, csrc/json_tp.h) through the C ABI: the default cf_toon_host
 path (token-parallel + sequential hand-over) must equal the sequential encoder (CF_TOON_SEQUENTIAL) unit for unit on a
 seeded fuzz corpus, and the tabular bench shape must stay on the fast path."""
-import ctypes
 import json
 import os
 import random
 import sys
 
-import numpy as np
 import pytest
 
 from mcp_context_forge_b200 import engine, synth
@@ -24,18 +22,8 @@ def toon(texts, flags):
     ctx = engine.Context.get()
     enc = [engine.encode_unit(t) for t in texts]
     stream, offs = engine.pack_units(enc)
-    batch = engine.Batch(ctx, len(stream), len(enc))
-    n = len(enc)
-    out = np.zeros(max(len(stream), 1), dtype=np.uint8)
-    out_len = np.zeros(n, dtype=np.uint32)
-    status = np.zeros(n, dtype=np.int32)
-    ctx.check(ctx.lib.cf_toon_host(ctx.h, batch.h, flags, ctypes.cast(ctypes.c_char_p(stream), ctypes.c_void_p), len(stream), offs.ctypes.data, n, out.ctypes.data,
-                                   out_len.ctypes.data, status.ctypes.data), "cf_toon_host")
-    res = []
-    for i in range(n):
-        o = int(offs[i])
-        res.append((int(status[i]), out[o:o + int(out_len[i])].tobytes() if status[i] == 0 else None))
-    return res, status, out_len
+    status, got, out_len = engine.toon_host_flags(engine.Batch(ctx, len(stream), len(enc)), stream, offs, flags)
+    return [(int(s), g) for s, g in zip(status, got)], status, out_len
 
 
 @pytest.mark.parametrize("rep", [0, 1])

@@ -3,11 +3,9 @@ substitution kernel, every scalar in every quoting-relevant TOON position on fou
 lane-window offset through the TOON and masking kernels, and the masking kernel's escaping, key order, key classes and
 non-JSON probes.  The corpora and CPython's answers come from test_unicode_sweep_cpu.py; nothing here is compared with
 another GPU path.  Each test prints its counts."""
-import ctypes
 import re
 import time
 
-import numpy as np
 import pytest
 
 import test_unicode_sweep_cpu as U
@@ -118,18 +116,8 @@ def toon_call(ctx, docs, flags):
     res, lens = [], []
     for part in chunks(docs):
         stream, offs = engine.pack_units(part)
-        n = len(part)
-        batch = engine.Batch(ctx, len(stream), n)
-        out = np.empty(max(len(stream), 1), dtype=np.uint8)
-        out_len = np.empty(n, dtype=np.uint32)
-        status = np.empty(n, dtype=np.int32)
-        with ctx.lock:
-            ctx.check(ctx.lib.cf_toon_host(ctx.h, batch.h, flags, ctypes.cast(ctypes.c_char_p(stream), ctypes.c_void_p), len(stream),
-                                           offs.ctypes.data, n, out.ctypes.data, out_len.ctypes.data, status.ctypes.data), "cf_toon_host")
-        raw = out.tobytes()
-        for i in range(n):
-            o = int(offs[i])
-            res.append((int(status[i]), raw[o:o + int(out_len[i])].decode("utf-8") if status[i] == 0 else None))
+        status, texts, out_len = engine.toon_host_flags(engine.Batch(ctx, len(stream), len(part)), stream, offs, flags)
+        res += [(int(s), None if t is None else t.decode("utf-8")) for s, t in zip(status, texts)]
         lens += out_len.tolist()
     return res, lens
 

@@ -9,7 +9,6 @@ With --record the reference itself is run and its answers are stored (tools/ref_
 with hand-over (with and without CF_TOON_REPORT_ERRORS) and token-parallel alone (CF_TOON_NO_HANDOVER), and cf_run_batch(CF_STAGE_TOON), each
 against the reference's answer under the product's strictly-smaller rule.
 usage: python tools/fuzz_vs_reference.py [seed] [cases] [gen1|gen2|synth] [--record | --device] [--answers NAME]"""
-import ctypes
 import importlib.util
 import json
 import math
@@ -147,18 +146,9 @@ REPORT_ERRORS, SEQUENTIAL, NO_HANDOVER, HANDED_OVER, FB_NUM_EXACT = 1, 8, 16, 7,
 
 def device_toon(engine, texts, flags):
     """cf_toon_host over `texts` as one batch: [(status, text or None)] and out_len (the hand-over reason under CF_TOON_NO_HANDOVER)."""
-    import numpy as np
-
-    ctx = engine.Context.get()
     stream, offs = engine.pack_units(texts)
-    n = len(texts)
-    out = np.zeros(max(len(stream), 1), dtype=np.uint8)
-    out_len = np.zeros(n, dtype=np.uint32)
-    status = np.zeros(n, dtype=np.int32)
-    batch = engine.Batch(ctx, len(stream), n)                  # held for the call: the handle is freed with the object
-    ctx.check(ctx.lib.cf_toon_host(ctx.h, batch.h, flags, ctypes.cast(ctypes.c_char_p(stream), ctypes.c_void_p), len(stream),
-                                   offs.ctypes.data, n, out.ctypes.data, out_len.ctypes.data, status.ctypes.data), "cf_toon_host")
-    return [(int(s), out[int(o):int(o) + int(k)].tobytes().decode("utf-8", "surrogateescape") if s == 0 else None) for s, o, k in zip(status, offs, out_len)], out_len
+    status, got, out_len = engine.toon_host_flags(engine.Batch(engine.Context.get(), len(stream), len(texts)), stream, offs, flags)
+    return [(int(s), None if g is None else g.decode("utf-8", "surrogateescape")) for s, g in zip(status, got)], out_len
 
 
 def device_run_batch(engine, texts, flags):
